@@ -1,11 +1,11 @@
-"""`FeMaSRNet` behind the reference's ARCH_REGISTRY surface, executed by the B200-native engine.
+"""`FeMaSRNet` behind the reference's ARCH_REGISTRY surface, executed by the H100-native engine.
 
 Drop-in for /root/reference/basicsr/archs/femasr_arch.py:214-479: same class name and registry key,
 same keyword-only constructor, same state_dict keys and shapes (SURVEY.md 8b), same method signatures
 and return tuples.  The module only HOLDS the parameters (so `.to()`, `.eval()`, `load_state_dict`,
 `state_dict` behave as usual); all arithmetic of forward / encode_and_decode / test / test_tile /
-decode_indices runs in libfemasr_b200.so (hand-written sm_100a CUDA) through `femasr_b200.net`.
-There is no CPU or eager-PyTorch fallback: calling the network without a CUDA sm_100 device raises.
+decode_indices runs in libfemasr_b200.so (hand-written sm_90a CUDA) through `femasr_b200.net`.
+There is no CPU or eager-PyTorch fallback: calling the network without a CUDA sm_90 (H100) device raises.
 
 In scope: norm_type 'gn', act_type 'silu'; one codebook at scale 32 or the multi-scale variant with further codebooks
 at 64 / 128 (femasr_arch.py:280-299); LQ_stage=True with scale_factor 2 or 4 (the SR network) and LQ_stage=False (the

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py - images/sec of the FeMaSR x4 SR hot path (BASELINE.json metric) on N B200s.
+"""bench.py - images/sec of the FeMaSR x4 SR hot path (BASELINE.json metric) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config 2|3|5|2test]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config 2|3|5|2test] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A step = one encode_and_decode pass (`FeMaSRNet.forward`) over one batch of synthetic LR images:
@@ -19,6 +19,9 @@ test_tile(256,32) on one 1024x1024 image; 2test: config 2 through FeMaSRNet.test
             launching stream (engine profile mode, extra steps after the timed region)
   cpu_baseline  the CPU oracle port (the reference's ATen-CPU arithmetic) on this host's cores, bounded sample
 --impl reference runs only that CPU arm as the step and prints the same line shape.
+--dump-outputs DIR writes what the last timed step returned as DIR/<name>.npy (with N GPUs: rank 0's view, i.e. the
+all-gathered SR batch and rank 0's own indices / loss), so that two builds can be compared output for output: weights
+and inputs depend only on the arguments.
 """
 from __future__ import annotations
 
@@ -36,7 +39,7 @@ if ROOT not in sys.path:
 
 METRIC = "images/sec x4 SR 128->512 batch32"
 GFLOP_PER_IMAGE = 754.53      # algorithmic, SURVEY.md 8d / BASELINE.md section 2 (x4 128x128 forward, e256)
-# BASELINE.json configs; "2" is the one the metric is quoted on, the others print the same line shape for profiles/
+# BASELINE.json configs; "2" is the one the metric is quoted on, the others print the same line shape
 CONFIGS = {
     "2": {"scale": 4, "lr": 128, "batch": 32, "entry": "forward", "name": "config 2"},
     "2test": {"scale": 4, "lr": 128, "batch": 32, "entry": "test", "name": "config 2 through test() (flip-pad to 144)"},
@@ -52,8 +55,8 @@ def load_peaks():
         d = json.load(open(p))
         return {"tflops_burst": d.get("bf16_tflops"), "tflops_sustained": d.get("bf16_tflops_sustained"),
                 "hbm_gbs": d.get("hbm_gbs"), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"tflops_burst": 1590.0, "tflops_sustained": 1400.0, "hbm_gbs": 6650.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"tflops_burst": 989.0, "tflops_sustained": None, "hbm_gbs": 3350.0,
+            "source": "H100 SXM data sheet, dense BF16 at 700 W (not measured)"}
 
 
 class ClockSampler:
@@ -180,6 +183,33 @@ def cpu_arm(args, steps: int, warmup: int, budget_s: float = 25.0):
     return ips, total / steps * 1e3, sample_b, info
 
 
+DUMP_MAX_BYTES = 48 << 20     # an output larger than this is dumped as a fixed seeded sample (all dumps stay < 64 MB)
+DUMP_SAMPLE = 2 << 20
+
+
+def dump_outputs(out_dir: str, arrays: dict):
+    """DIR/<name>.npy (float32; integer data as float64); a large output as a fixed seeded sample + its flat indices."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        if t is None:
+            continue
+        ts = t if isinstance(t, (list, tuple)) else [t]
+        for k, v in enumerate(ts):
+            key = name if len(ts) == 1 else f"{name}{k}"
+            v = v.detach()
+            v = v.double() if not v.is_floating_point() else v.float()
+            flat = v.reshape(-1)
+            if flat.numel() * flat.element_size() > DUMP_MAX_BYTES:
+                g = torch.Generator().manual_seed(0)
+                idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+                np.save(os.path.join(out_dir, f"{key}_sample_index.npy"), idx.double().numpy())
+                np.save(os.path.join(out_dir, f"{key}_sample.npy"), flat[idx.to(flat.device)].cpu().numpy())
+            else:
+                np.save(os.path.join(out_dir, f"{key}.npy"), v.cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -193,6 +223,8 @@ def main():
     ap.add_argument("--e-dim", type=int, default=256)
     ap.add_argument("--gemm-path", type=int, default=None)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (rank 0; SR batch all-gathered)")
     args = ap.parse_args()
     cfgd = CONFIGS[args.config]
     args.batch = args.batch or cfgd["batch"]
@@ -224,7 +256,7 @@ def main():
               "lr_size": args.lr, "scale": args.scale, "codebook": [1024, args.e_dim],
               "parallelism": (f"dp{world} (batch shards; one NCCL all-gather of the output shards per step on a side stream, "
                               "overlapping the next step's forward; drained inside the timed region)") if world > 1 else "single GPU",
-              "l2": "no explicit flush: per-step working set (2.1 GB per decoder tensor at batch 32) >> 126 MB L2",
+              "l2": "no explicit flush: per-step working set (2.1 GB per decoder tensor at batch 32) >> 50 MB L2",
               "launch": "CUDA graph replay of the engine's launch list" if os.environ.get("FEMASR_CUDA_GRAPH", "1") != "0" else "eager launches"}
 
     # ------------------------------------------------------------------ reference arm (CPU)
@@ -240,7 +272,7 @@ def main():
         emit(line)
         return 0
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     import torch
     import torch.distributed as dist
     from basicsr.archs import build_network
@@ -248,7 +280,7 @@ def main():
     from femasr_b200.spec import random_state_dict
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py --impl b200 needs a CUDA sm_100 device (no CPU fallback)")
+        raise SystemExit("bench.py --impl b200 needs a CUDA sm_90 (H100) device (no CPU fallback)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -266,14 +298,18 @@ def main():
     y_host = torch.empty(B, 3, S * args.scale, S * args.scale).pin_memory()
     eng = net._native(dev)
 
+    last = {}            # what the most recent resident step returned, by name (--dump-outputs)
+
     def run_resident():
         """One pass of the configuration's entry over the device-resident batch -> SR tensor."""
         if args.entry == "forward":
             # the engine's fixed launch list, replayed as a CUDA graph (same kernels, no per-launch host work)
-            return (eng.forward_graph(x_dev) if eng.use_graph else eng.forward(x_dev, want_indices=True, want_loss=True))[0]
-        if args.entry == "test":
-            return eng.test(x_dev)
-        return eng.test_tile(x_dev, TILE, TILE_PAD)
+            y, loss, idx = eng.forward_graph(x_dev) if eng.use_graph else eng.forward(x_dev, want_indices=True, want_loss=True)
+            last.update(sr=y, loss=loss, indices=idx)
+            return y
+        y = eng.test(x_dev) if args.entry == "test" else eng.test_tile(x_dev, TILE, TILE_PAD)
+        last.update(sr=y)
+        return y
 
     def run_public(xd):
         """The same through the reference-facing surface (what a user of FeMaSRNet calls)."""
@@ -382,6 +418,10 @@ def main():
         sampler.start()
     ms_total = timed(step_resident, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        if gather:
+            last["sr"] = gather.full[(gather.i - 1) & 1]     # the all-gathered batch of the last step (drained above)
+        dump_outputs(args.dump_outputs, last)
     # one eager pass with the engine's profile mode on: counts the kernels one step launches (and their FLOPs)
     eng.set_profile(True)
     if args.entry == "forward":
@@ -427,24 +467,15 @@ def main():
     achieved = d["flops"] / (d["ms"] / 1e3) / 1e12 if d["ms"] > 0 else 0.0
     peak = peaks["tflops_sustained"] or peaks["tflops_burst"]
     tot_ms = sum(v["ms"] for v in prof.values())
-    traffic, traffic_src = None, None
-    tps = [os.path.join(ROOT, "profiles", f"tc_igemm_traffic_r{r}.json") for r in (2, 1)]
-    tp = next((t for t in tps if os.path.exists(t)), None)
-    if dname == "tc_igemm" and tp and args.config == "2":
-        tj = json.load(open(tp))
-        traffic = int(tj["dram_bytes_per_launch"])
-        traffic_src = (f"profiles/{os.path.basename(tp)}: ncu dram__bytes_read.sum+dram__bytes_write.sum averaged over the "
-                       f"{tj['launches']} tc_igemm launches of one batch-32 step (L2->SM traffic is "
-                       f"{tj['l2_bytes_total'] / (tj['dram_read_bytes_total'] + tj['dram_write_bytes_total']):.1f}x that: the kernel is L2-bandwidth bound)")
     roofline = {"bound": "tensor", "kernel": dname, "achieved": round(achieved, 2), "peak": peak, "unit": "TFLOP/s",
-                "frac": round(achieved / peak, 4), "traffic": traffic, "traffic_source": traffic_src,
-                "peak_source": peaks["source"] + ", cuBLAS bf16 sustained (kernel timed inside a long step)",
+                "frac": round(achieved / peak, 4), "traffic": None, "traffic_source": None,
+                "peak_source": peaks["source"],
                 "launches_per_step": d["launches"] // 2, "avg_launch_ms": round(d["ms"] / max(1, d["launches"]), 4),
                 "share_of_step": round(d["ms"] / tot_ms, 4) if tot_ms else None,
                 "flops_counted": "algorithmic 2*MAC of the convs/linears this kernel executed",
                 "arithmetic": "fp32 FFMA (SIMT)" if gemm_path == 0 else (
-                    "tcgen05, fp32 accumulate in TMEM; in front of the VQ 3-MMA split-fp16 kind::f16 (hi*hi+hi*lo+lo*hi); behind it "
-                    + ("a_hi*w_hi on kind::f16 + ONE kind::f8f6f4 e4m3 product for both cross terms (2.0 MMA units per algorithmic MMA)"
+                    "wgmma (sm_90a), fp32 accumulate in registers; in front of the VQ 3 split-fp16 products (hi*hi+hi*lo+lo*hi); behind it "
+                    + ("a_hi*w_hi in fp16 + ONE e4m3 product of twice the K for both cross terms (2.0 MMA units per algorithmic MMA)"
                        if os.environ.get("FEMASR_F8_CROSS", "1") != "0" else "the same 3 products")),
                 "path_tflops": round(flops_step / (ms_step / 1e3) / 1e12, 2),
                 "path_frac": round(flops_step / (ms_step / 1e3) / 1e12 / peak, 4),

@@ -1,4 +1,4 @@
-"""femasr_b200: B200-native (sm_100a) implementation of FeMaSR's inference hot path.
+"""femasr_b200: H100-native (sm_90a) implementation of FeMaSR's inference hot path.
 
   femasr_b200.lib    ctypes binding of libfemasr_b200.so (C ABI in include/femasr_b200.h)
   femasr_b200.net    host engine wrapper (workspace, test()/test_tile() scheduling)
@@ -12,6 +12,6 @@ __version__ = "0.1.0"
 
 
 def default_gemm_path() -> int:
-    """1 = tcgen05 split-fp16 tensor-core GEMM (default), 0 = fp32 SIMT implicit GEMM (exact-arithmetic
+    """1 = wgmma split-fp16 tensor-core GEMM (default), 0 = fp32 SIMT implicit GEMM (exact-arithmetic
     debug path); FEMASR_GEMM_PATH overrides."""
     return int(os.environ.get("FEMASR_GEMM_PATH", "1"))

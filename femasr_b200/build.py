@@ -1,8 +1,9 @@
-"""Build libfemasr_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libfemasr_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m femasr_b200.build [--force]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and the object files are build products (git-ignored); `build()` recompiles them whenever a source, a header or
+the flags change.
 """
 from __future__ import annotations
 
@@ -19,8 +20,9 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libfemasr_b200.so")
 
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *ARCH,
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC,-O2,-fvisibility=default",
     "-I", os.path.join(ROOT, "include"), "-I", CSRC,
@@ -66,7 +68,7 @@ def build_variant(out_name: str, defines, verbose: bool = False) -> str:
             print(r.stderr)
         objs.append(obj)
     out = os.path.join(HERE, out_name)
-    r = subprocess.run([nvcc, "-shared", "-o", out, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"],
+    r = subprocess.run([nvcc, "-shared", "-o", out, *objs, *ARCH, "-lcudart"],
                        capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
@@ -98,7 +100,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(compile_one, srcs))
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, *ARCH, "-lcudart"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -84,11 +84,11 @@ __global__ void __launch_bounds__(64) window_attention_kernel(const float* __res
 
 // ------------------------------------------------------------------------------------------------
 // Tensor-core variant (warp-level mma.sync m16n8k16, fp16 operands split hi/lo, fp32 accumulate): the
-// 64x32x64 per-(window, head) products are far too small for a tcgen05 tile, so the legacy warp MMA path is
+// 64x32x64 per-(window, head) products are far too small for a 128-row wgmma tile, so the legacy warp MMA path is
 // the right tool here.  One CTA of 4 warps per (window, head); warp w owns query rows [16w, 16w+16).
 //   S = (q*scale) K^T  -> + rel-pos bias (+ shift mask) -> softmax (fp32, in registers) -> O = P V.
 // Both products use the same 3-term split as the big GEMMs (lo*hi + hi*lo + hi*hi).
-// The kernel is bound by the LSU data pipe (ncu: l1tex wavefronts 91 %), so every access is shaped to need few of them:
+// The kernel is bound by the LSU data pipe, so every access is shaped to need few of them:
 //   * K / V rows are fetched with 8 consecutive lanes per 128-byte row and kept ROW-MAJOR in shared memory; the
 //     B fragments come from ldmatrix.x4 (K) and ldmatrix.x4.trans (V) - no transposing 2-byte stores;
 //   * the head dimension of Q and K is permuted (the contraction order of an MMA is free as long as both operands
@@ -121,8 +121,8 @@ __device__ __forceinline__ void split2(float x, float y, uint32_t& hi, uint32_t&
 
 constexpr int KV_LD = 40;   // row stride in halves (80 B): the 8 row addresses of an ldmatrix phase hit 8 distinct 16-byte slots
 
-// 7 resident CTAs per SM (72 registers): measured 0.139 ms per layer vs 0.141 at 6 (80 registers) and 0.181 when the
-// compiler is left free to use more registers
+// 7 resident CTAs per SM (72 registers): more CTAs in flight hide the shared-memory latency better than the registers
+// a freer allocation would save
 #ifndef FEMASR_ATTN_MINBLOCKS
 #define FEMASR_ATTN_MINBLOCKS 7
 #endif

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libfemasr_b200 (sm_100a).
+// Shared host/device helpers for libfemasr_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -53,7 +53,7 @@ inline int sm_count() {
   if (!counts[d]) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d);
-    counts[d] = n > 0 ? n : 148;
+    counts[d] = n > 0 ? n : 132;
   }
   return counts[d];
 }

@@ -294,7 +294,7 @@ struct Ctx {
   }
 
   // tensor-core variant of conv(): stage the activation operand (prologue + fp16 split) unless the producer
-  // already wrote split planes (pre_hi/pre_lo), then the tcgen05 implicit GEMM; optionally the result is
+  // already wrote split planes (pre_hi/pre_lo), then the wgmma implicit GEMM; optionally the result is
   // emitted as split planes for the next GEMM (out_hi/out_lo) instead of fp32 y.  A fused nearest-x2 upsample
   // runs as four sub-pixel 2x2 convs on the low-res operand.  Allocation happens in dry runs too.
   void conv_tc(const std::string& wname, const float* x, float* y, int B, int Hin, int Win, int Cin, int Cout, int ksize,
@@ -339,7 +339,7 @@ struct Ctx {
       const int slice = net->tc_slice_kb;        // k-blocks per accumulator drain (default 4 = 256 of K)
       if ((precise || precise_region) && net->tc_precise && nkb > slice) {
         // K-sliced accumulation (layers in front of the VQ): every 256 of K the tensor core's truncating accumulator
-        // is folded into an fp32 round-to-nearest running sum held in TMEM (see femasr_tc_args.slice_kb)
+        // is folded into an fp32 round-to-nearest running sum held in registers (see femasr_tc_args.slice_kb)
         t.slice_kb = slice;
       }
       run(detail_name("tc_igemm", ksize, Cin, Cout, Hin, Win, upsample, stride, t.slice_kb), flops,

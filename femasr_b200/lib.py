@@ -1,7 +1,7 @@
 """ctypes binding of libfemasr_b200.so (the C ABI declared in include/femasr_b200.h).
 
 There is no CPU fallback: loading fails loudly if the library has not been built, and every
-compute entry point returns an error without an sm_100 device.
+compute entry point returns an error without an sm_90 (H100) device.
 """
 from __future__ import annotations
 
@@ -147,10 +147,10 @@ def check(status: int) -> None:
 
 
 def require_device() -> int:
-    """Compute capability of the current device; raises unless it is sm_100."""
+    """Compute capability of the current device; raises unless it is sm_90 (the library is built for sm_90a only)."""
     cc = load().femasr_device_cc()
     if cc < 0:
         check(cc)
-    if cc // 10 != 10:
-        raise FemasrError(f"femasr_b200 kernels are built for sm_100a only; current device is sm_{cc}")
+    if cc != 90:
+        raise FemasrError(f"femasr_b200 kernels are built for sm_90a only; current device is sm_{cc}")
     return cc

@@ -1,4 +1,4 @@
-"""Host side of the B200-native FeMaSR path: owns the C engine handle, the device workspace and the
+"""Host side of the H100-native FeMaSR path: owns the C engine handle, the device workspace and the
 test()/test_tile() scheduling.  PyTorch is used for device memory and the current stream only; all
 arithmetic happens in libfemasr_b200.so through the C ABI (include/femasr_b200.h).
 
@@ -81,7 +81,7 @@ class NativeNet:
     # ------------------------------------------------------------------ lifecycle
     def _ensure(self, device: torch.device):
         if device.type != "cuda":
-            raise L.FemasrError("femasr_b200 runs on a CUDA sm_100 device only (no CPU fallback); "
+            raise L.FemasrError("femasr_b200 runs on a CUDA sm_90 (H100) device only (no CPU fallback); "
                                 f"got tensors on '{device}'")
         if self._h.value is None:
             with torch.cuda.device(device):

@@ -50,7 +50,7 @@ def all_gather_outputs(local: torch.Tensor, counts: List[int], group: Optional[d
 class PeerGather:
     """All-gather of EQUAL output shards by copy-engine peer writes instead of an NCCL kernel (one node, one process per GPU).
 
-    Why: the tensor-core kernels of this path are persistent - 148 CTAs, one per SM, each with a STATIC share of the tiles
+    Why: the tensor-core kernels of this path are persistent - 132 CTAs, one per SM, each with a STATIC share of the tiles
     and the whole 227 KB of shared memory.  An NCCL all-gather kernel that overlaps them (side stream) takes a few SMs for
     its own CTAs; the tc_igemm CTAs that find no SM start only when another CTA of the same launch has finished its share,
     so every launch in that window runs for up to two shares.  Peer-to-peer `cudaMemcpyAsync` over NVLink runs on the DMA

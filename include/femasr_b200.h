@@ -1,6 +1,6 @@
-/* femasr_b200.h - C ABI of the B200-native FeMaSR inference hot path.
+/* femasr_b200.h - C ABI of the H100-native FeMaSR inference hot path.
  *
- * This shared library (libfemasr_b200.so, sm_100a only) is the drop-in boundary underneath the
+ * This shared library (libfemasr_b200.so, sm_90a only) is the drop-in boundary underneath the
  * reference's Python operator surface `basicsr.archs.femasr_arch.FeMaSRNet`
  * (/root/reference/basicsr/archs/femasr_arch.py:214-479).  Signatures use plain pointers and
  * sizes only: device pointers are raw CUDA addresses, `stream` is a cudaStream_t passed as void*.
@@ -25,7 +25,7 @@ typedef enum {
   FEMASR_ERR_ARG = -1,       /* bad shape / null pointer / unsupported configuration */
   FEMASR_ERR_CUDA = -2,      /* a CUDA runtime/driver call failed */
   FEMASR_ERR_STATE = -3,     /* missing parameter, workspace too small, ... */
-  FEMASR_ERR_NO_DEVICE = -4  /* no sm_100 device: there is no CPU fallback */
+  FEMASR_ERR_NO_DEVICE = -4  /* no sm_90 device: there is no CPU fallback */
 } femasr_status;
 
 const char* femasr_last_error(void);
@@ -49,7 +49,7 @@ typedef struct {
   int in_channel;     /* 3 */
   int use_quantize;   /* femasr_arch.py:224,349-350: 0 => z_quant = feat_to_quant (VQ still runs) */
   int use_residual;   /* femasr_arch.py:226,361-362 */
-  int gemm_path;      /* 0 = fp32 SIMT implicit GEMM, 1 = tcgen05 split-fp16 tensor-core GEMM */
+  int gemm_path;      /* 0 = fp32 SIMT implicit GEMM, 1 = wgmma split-fp16 tensor-core GEMM */
   /* multi-scale codebooks (femasr_arch.py:231-235, 280-299): rows of codebook_params.  n_codebooks 0 or 1 = the single
    * codebook (32, n_e, e_dim) above; else cb_scale[0] must be 32 (it fixes the depth, :255-256), the others an
    * increasing subset of {64, 128}; n_e / e_dim above are ignored. */
@@ -168,9 +168,9 @@ typedef struct {
 } femasr_igemm_args;
 int femasr_igemm_simt(const femasr_igemm_args* a, void* stream);
 
-/* ---- tcgen05 tensor-core implicit GEMM (gemm_path 1): same contract as femasr_igemm_simt for ksize 1|3,
+/* ---- wgmma tensor-core implicit GEMM (gemm_path 1): same contract as femasr_igemm_simt for ksize 1|3,
  * stride 1, Cin%64==0, Cout%64==0, computed as a 3-product split-fp16 GEMM (a_hi*w_hi + a_hi*w_lo + a_lo*w_hi,
- * fp32 accumulate in TMEM).  The activation operand is staged once per layer as two fp16 NHWC planes by
+ * fp32 accumulate in registers).  The activation operand is staged once per layer as two fp16 NHWC planes by
  * femasr_tc_prepare (which also applies the GN+SiLU / LayerNorm prologue and the nearest x2 upsample);
  * weights are packed once by femasr_tc_pack_weight into a blob of femasr_tc_weight_bytes bytes. */
 typedef struct {
@@ -192,12 +192,10 @@ typedef struct {
                               by the caller in fp32 (round-to-nearest) by chaining launches with res1 = y, which bounds
                               the tensor-core accumulator's truncation error to one slice */
   int slice_kb;            /* >0: the same slicing inside ONE launch - every slice_kb k-blocks the MMA accumulator is
-                              drained into an fp32 running sum held in the second TMEM buffer (tcgen05.ld/st, RN adds) */
-  int pair;                /* 1: CTA pairs (tcgen05 cta_group::2, 256-row tiles, each CTA stages half the weight tile);
-                              0: single-CTA tiles; -1: library default */
-  int strip;               /* 1: row-strip tiles (one image row of 128 pixels; the three horizontal taps share one
-                              130-pixel activation strip in shared memory): plain 3x3 stride-1 convs, Cout tile <= 128,
-                              W >= 128, no K slicing.  0: off; -1: automatic */
+                              folded into an fp32 running sum held in registers (RN adds) */
+  int pair;                /* schedule hints of other GPU generations (CTA-pair tiles, row-strip tiles): accepted for ABI
+                              compatibility (1 / 0 / -1 = default) and ignored by the sm_90a kernel, which has one */
+  int strip;               /* tile schedule; results do not depend on either */
   float* gn_partial;       /* optional: GroupNorm(32) partial sums of the OUTPUT, [B][rows][32][2] fp32 with
                               rows = femasr_tc_gn_partial_rows(args); finished by femasr_gn_finalize_rows */
   int upsample;            /* 1: y [B,2H,2W,Cout] = conv3x3(nearest_x2(a)), evaluated as 4 sub-pixel 2x2 convs on the
@@ -205,7 +203,7 @@ typedef struct {
   int f8;                  /* 1: F8 cross-term mode (layers behind the VQ, error budget 1e-3 on the output): a_lo and the
                               blob's second plane hold interleaved e4m3 bytes (femasr_tc_prepare_f8 /
                               femasr_tc_pack_weight_f8) and the two cross products a_lo*w_hi + a_hi*w_lo run as ONE
-                              kind::f8f6f4 product at twice the fp16 rate: 2.0 instead of 3.0 MMA units per k-step */
+                              e4m3 wgmma of twice the K at twice the fp16 rate: 2.0 instead of 3.0 MMA units per k-step */
 } femasr_tc_args;
 size_t femasr_tc_weight_bytes(int Cout, int Cin, int kh, int kw);
 int femasr_tc_pack_weight(const float* w_oihw, void* blob, int Cout, int Cin, int kh, int kw, void* stream);
@@ -267,7 +265,7 @@ int femasr_vq_select(const float* z, const float* zc, const float* codebook, con
 /* Fused VQ feature matching on the tensor cores (femasr_arch.py:35-38, 50-100) - the [N, n_e] distance matrix and the
  * one-hot of the reference never exist:
  *   femasr_vq_match_tc  z (split fp16 planes [N, e_dim]) x codebook (femasr_tc_pack_weight blob of the [n_e, e_dim]
- *                       embedding) on tcgen05; the epilogue evaluates d_j = fl(fl(A + B_j) - 2 C_j) and keeps per row the
+ *                       embedding) on the tensor cores (wgmma); the epilogue evaluates d_j = fl(fl(A + B_j) - 2 C_j) and keeps per row the
  *                       four smallest (d, j) in cand[N][4] = {float bits, int32} pairs, ascending.  a = row_sumsq(z),
  *                       esq = row_sumsq(codebook).
  *   femasr_vq_finish    exact fp32 re-evaluation of the candidates that lie within rounding distance of the best

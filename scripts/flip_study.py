@@ -20,11 +20,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 VARIANTS = {
-    "default (tcgen05, K-slice 256)": {},
-    "tcgen05, K-slice 128": {"FEMASR_TC_SLICE_KB": "2"},
-    "tcgen05, K-slice 64": {"FEMASR_TC_SLICE_KB": "1"},
-    "tcgen05, no K-slicing": {"FEMASR_TC_PRECISE": "0"},
-    "tcgen05, VQ on fp32 SIMT": {"FEMASR_VQ_FUSED": "0"},
+    "default (tensor-core, K-slice 256)": {},
+    "tensor-core, K-slice 128": {"FEMASR_TC_SLICE_KB": "2"},
+    "tensor-core, K-slice 64": {"FEMASR_TC_SLICE_KB": "1"},
+    "tensor-core, no K-slicing": {"FEMASR_TC_PRECISE": "0"},
+    "tensor-core, VQ on fp32 SIMT": {"FEMASR_VQ_FUSED": "0"},
     "fp32 FFMA path (gemm_path=0)": {"FEMASR_GEMM_PATH": "0"},
 }
 

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Full validation + evidence pass on the GPU box (one B200): tests, bench lines, per-layer table, sanitizer, ncu launch
+# Full validation + evidence pass on one GPU: tests, bench lines, per-layer table, sanitizer, ncu launch
 # list and DRAM/L2 traffic of the dominant kernel.  Outputs under gpurun_out/ (tag = $1, default "final").
 set -u
 cd "$(dirname "$0")/.."

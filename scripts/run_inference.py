@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Folder / single-image super-resolution with the B200-native FeMaSRNet.
+"""Folder / single-image super-resolution with the H100-native FeMaSRNet.
 
 Same command line and behaviour as the reference's demo entry point (inference_femasr.py:19-69: -i/-w/-o/-s/
 --suffix/--max_size; images below max_size^2 pixels go through `test`, larger ones through `test_tile`), written

@@ -1,7 +1,7 @@
 #!/bin/bash
 # compute-sanitizer memcheck + racecheck + synccheck over one small forward per GEMM path (GPU box).
-# The input (1x3x32x128, x4) reaches every tcgen05 variant: CTA pairs (256-wide long-K convs), row strips with
-# streamed (128ch @64x256) and resident (64ch @128x512) weights, K-sliced accumulation (layers in front of the VQ),
+# The input (1x3x32x128, x4) reaches every tensor-core GEMM variant: 64- and 128-wide tiles, K-sliced accumulation
+# (layers in front of the VQ), F8 cross terms (behind it),
 # sub-pixel upsample convs, stride-2 TMA, split-plane outputs, GroupNorm partials; plus attention / VQ / edge kernels.
 # Usage: bash scripts/run_sanitizer.sh   -> gpurun_out/sanitizer_*.txt + gpurun_out/sanitizer_summary.txt
 set -u

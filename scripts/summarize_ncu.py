@@ -1,4 +1,4 @@
-"""Summarise ncu CSV logs into the small committed files under profiles/.
+"""Summarise ncu CSV logs into small summary files (a launch table, or the DRAM / L2 traffic of one step).
   python scripts/summarize_ncu.py launches <csv> <out.csv> "<title>"
   python scripts/summarize_ncu.py traffic  <csv> <out.json>"""
 import collections

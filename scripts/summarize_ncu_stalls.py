@@ -2,7 +2,7 @@
 """Summarise `ncu --set full --import-source on` captures of single kernels (read here, without a GPU):
 headline raw metrics + warp-stall sampling per reason + the instructions with the most samples.
 
-    python scripts/summarize_ncu_stalls.py name=gpurun_out/prof_x.ncu-rep ... > profiles/ncu_r2_stalls.json
+    python scripts/summarize_ncu_stalls.py name=prof_x.ncu-rep ... > ncu_stalls.json
 """
 import csv
 import io

@@ -10,7 +10,7 @@ sys.dont_write_bytecode = True
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA sm_100 device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA sm_90 (H100) device")
 
 
 @pytest.fixture(scope="session")

@@ -142,6 +142,23 @@ def main():
         path = os.path.join(sub, name + ".npz")
         np.savez_compressed(path, **rec)
         print(f"{name}: out {tuple(out.shape)} |out|max {out.abs().max():.3f}  -> {os.path.getsize(path) / 1e3:.0f} kB")
+    state_dict_inventory(ref)
+
+
+def state_dict_inventory(ref):
+    """reference_state_dicts.json.gz: name -> [shape, dtype] of the reference's state_dict() for every configuration of
+    tests/test_boundary.py (which checks femasr_b200.spec and the drop-in module against it)."""
+    import gzip
+    import json
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_boundary import CONFIGS, IDS
+    inv = {}
+    for (scale, cbs), cid in zip(CONFIGS, IDS):
+        net = ref.FeMaSRNet(codebook_params=cbs, LQ_stage=scale != 1, scale_factor=scale)
+        inv[cid] = {k: [list(v.shape), str(v.dtype).replace("torch.", "")] for k, v in net.state_dict().items()}
+    text = json.dumps(inv, sort_keys=True, separators=(",", ":")) + "\n"
+    with gzip.GzipFile(os.path.join(OUT, "reference_state_dicts.json.gz"), "wb", compresslevel=9, mtime=0) as f:
+        f.write(text.encode())
 
 
 if __name__ == "__main__":

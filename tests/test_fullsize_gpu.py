@@ -4,8 +4,8 @@ script's default test_tile(240, 16) on a >600-pixel image), default init = the t
 the VQ stage has up to 131072 rows and 0.1-0.2 % of them are exact fp32 ties (SURVEY 7.3-2).
 
 Bars (north_star): codebook indices BIT-EXACT against the CPU oracle (which is pinned to the unmodified reference),
-output max-abs <= 1e-3.  Zero tolerance on both GEMM paths.  Every measured (flips, max-abs) pair is appended to
-gpurun_out/parity_report.json (copied to profiles/parity_r2.json)."""
+output max-abs <= 1e-3.  Zero tolerance on both GEMM paths.  With FEMASR_PARITY_REPORT=<file>, every measured
+(flips, max-abs) pair is also recorded in that JSON file."""
 import json
 import os
 
@@ -18,12 +18,12 @@ from femasr_b200.spec import random_state_dict
 from oracle import femasr_oracle as O
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REPORT = os.path.join(ROOT, "gpurun_out", "parity_report.json")
+REPORT = os.environ.get("FEMASR_PARITY_REPORT")
 
 
 def record(name, **fields):
-    os.makedirs(os.path.dirname(REPORT), exist_ok=True)
+    if not REPORT:
+        return
     data = {}
     if os.path.exists(REPORT):
         try:
@@ -91,7 +91,7 @@ def forced_indices(idx_forced):
 
 
 def test_config2_full_batch_against_oracle(cuda):
-    """BASELINE config 2 at its FULL size on the default (tcgen05) path: batch 32, 131072 VQ rows, every index and every
+    """BASELINE config 2 at its FULL size on the default (tensor-core) path: batch 32, 131072 VQ rows, every index and every
     output pixel against the CPU oracle (about a minute of host time).
 
     What can hold at this size.  With the default U(+-1/1024) codebook the fp32 distances sit on a grid of ulp(sum z^2)
@@ -100,7 +100,7 @@ def test_config2_full_batch_against_oracle(cuda):
     oracle is reproducible against itself (thread count / batch chunking: 0 of 131072, profiles/oracle_selfcheck_r2.json)
     but moves ~0.1-0.2 % of the rows against its own fp64 evaluation (same file; SURVEY 7.3-1), and any fp32 evaluation
     in another order - this engine's fp32-FFMA path as much as its tensor-core path - lands a handful of rows per 131072
-    on the other side of such a tie (profiles/flip_study_r2.json).  0 of 16384 (test above) is the practical form of
+    on the other side of such a tie (`scripts/flip_study.py` counts them).  0 of 16384 (test above) is the practical form of
     "bit-exact"; at 131072 rows the enforceable statement is:
       * at most 16 differing rows (1.2e-4; the oracle's own fp32-vs-fp64 rate is 10x that);
       * every differing row is TIE-EQUIVALENT under the oracle's own arithmetic: the oracle's fp32 distance of our code

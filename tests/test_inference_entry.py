@@ -1,5 +1,7 @@
-"""Config 1 plumbing (image folder -> PNGs): the reference's own entry script against this repo's surface on
-CPU (must get as far as the device check), and the demo entry on the GPU against the oracle."""
+"""Config 1 plumbing (image folder -> PNGs): the reference's own entry script (tests/fixtures/inference_femasr.py)
+against this repo's surface on CPU (must get as far as the device check), and the demo entry on the GPU against the
+oracle."""
+import hashlib
 import os
 import runpy
 import sys
@@ -12,9 +14,11 @@ import torch
 from basicsr.utils import img2tensor, tensor2img
 from femasr_b200.spec import random_state_dict
 from oracle import femasr_oracle as O
-from oracle.ref_shim import REFERENCE_ROOT, reference_available
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+FIXTURE = os.path.join(ROOT, "tests", "fixtures", "inference_femasr.py")
+# sha256 of the reference's inference_femasr.py (the unmodified upstream entry script)
+REFERENCE_SCRIPT_SHA256 = "35f0741be421aa418bc382360fe07f5d7f50c5b6aebb759e1fe5ae7bc7d17913"
 
 
 def _write_inputs(folder, sizes, seed=3):
@@ -39,7 +43,7 @@ def test_image_helpers_roundtrip():
     assert tensor2img(torch.full((1, 3, 2, 2), 1.7)).max() == 255     # clamp before scaling
 
 
-@pytest.mark.skipif(not reference_available() or torch.cuda.is_available(), reason="needs /root/reference and no GPU")
+@pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU behaviour")
 def test_reference_entry_script_runs_unchanged_up_to_the_device(tmp_path, built_lib):
     """inference_femasr.py of the reference, unmodified, imports our basicsr, builds and loads the network and
     reads the image; without a GPU it must stop exactly at the first compute call (no CPU fallback)."""
@@ -50,19 +54,16 @@ def test_reference_entry_script_runs_unchanged_up_to_the_device(tmp_path, built_
     argv = sys.argv
     sys.argv = ["inference_femasr.py", "-s", "4", "-i", ins[0], "-o", str(tmp_path / "out"), "-w", str(w)]
     try:
-        with pytest.raises(FemasrError, match="CUDA sm_100"):
-            runpy.run_path(os.path.join(REFERENCE_ROOT, "inference_femasr.py"), run_name="__main__")
+        with pytest.raises(FemasrError, match="CUDA sm_90"):
+            runpy.run_path(FIXTURE, run_name="__main__")
     finally:
         sys.argv = argv
 
 
-@pytest.mark.skipif(not reference_available(), reason="needs /root/reference")
 def test_fixture_is_the_reference_script():
-    """tests/fixtures/inference_femasr.py (what the GPU box executes, tests/test_reference_entry_gpu.py) must be the
-    reference's entry script byte for byte."""
-    a = open(os.path.join(ROOT, "tests", "fixtures", "inference_femasr.py"), "rb").read()
-    b = open(os.path.join(REFERENCE_ROOT, "inference_femasr.py"), "rb").read()
-    assert a == b
+    """tests/fixtures/inference_femasr.py (executed by tests/test_reference_entry_gpu.py) must be the reference's entry
+    script byte for byte."""
+    assert hashlib.sha256(open(FIXTURE, "rb").read()).hexdigest() == REFERENCE_SCRIPT_SHA256
 
 
 @pytest.mark.gpu

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 split-fp16 implicit GEMM (gemm_path 1) against fp64 ATen on CPU, through the C ABI,
+"""GPU: the wgmma split-fp16 implicit GEMM (gemm_path 1) against fp64 ATen on CPU, through the C ABI,
 and the whole network on that path against the reference goldens / the oracle.
 
 Accuracy bar for the kernel: the 3-product split carries ~22 significand bits per operand, so errors must
@@ -125,7 +125,7 @@ def test_tc_k_sliced_accumulation(cuda):
     res2 = res.clone()
     y3 = G.tc_igemm(hi, lo, blob, bg, Cout, 3, res1=res2, y=res2, slice_kb=4)      # in-kernel slicing, in-place residual
     e1, e2, e3 = rel_err(G.nchw(one), want), rel_err(G.nchw(y), want), rel_err(G.nchw(y3), want)
-    print(f"K=2304 conv: single pass rel err {e1:.2e}, K-sliced launches {e2:.2e}, in-kernel TMEM running sum {e3:.2e}")
+    print(f"K=2304 conv: single pass rel err {e1:.2e}, K-sliced launches {e2:.2e}, in-kernel running sum {e3:.2e}")
     assert e2 <= 2e-6 and e2 < e1
     assert e3 <= 2e-6 and e3 < e1
     # linear K=1024 (fc2-like) and a partial last slice (K = 9*128/64 = 18 k-blocks, slices of 4)
@@ -144,9 +144,10 @@ def test_tc_k_sliced_accumulation(cuda):
 @pytest.mark.parametrize("B,H,W,Cin,Cout,kw", [
     (1, 24, 40, 256, 256, {}), (2, 16, 24, 128, 128, {}), (1, 33, 17, 128, 64, {}), (3, 64, 64, 64, 64, {}),
     (1, 8, 8, 256, 256, {"upsample": 1}), (1, 31, 31, 256, 256, {"stride": 2}), (1, 24, 40, 256, 256, {"slice_kb": 4}),
-    (2, 16, 24, 128, 128, {"slice_kb": 4})])        # 128-wide: the three-buffer sliced protocol over a CTA pair
+    (2, 16, 24, 128, 128, {"slice_kb": 4})])        # 128-wide tiles, K-sliced accumulation
 def test_tc_cta_pair(cuda, B, H, W, Cin, Cout, kw):
-    """tcgen05 cta_group::2 variant (256-row tiles over a CTA pair, odd tile counts -> dummy second tile)."""
+    """Shape coverage against fp64: odd tile counts, sub-pixel phases, stride 2, K slicing, with femasr_tc_args.pair
+    both 0 and 1 (a schedule hint the sm_90a kernel accepts and ignores; each call must still be right)."""
     x, w, b = rnd(B, Cin, H, W, seed=46), rnd(Cout, Cin, 3, 3, seed=47, scale=0.03), rnd(Cout, seed=48)
     up, stride = kw.get("upsample", 0), kw.get("stride", 1)
     xin = O.upsample2(x) if up else x
@@ -157,19 +158,18 @@ def test_tc_cta_pair(cuda, B, H, W, Cin, Cout, kw):
     blob = G.tc_pack_up2(w.to(cuda)) if up else G.tc_pack(w.to(cuda))
     y1 = G.tc_igemm(hi, lo, blob, b.to(cuda), Cout, 3, res1=res.to(cuda), pair=0, **kw)
     y2 = G.tc_igemm(hi, lo, blob, b.to(cuda), Cout, 3, res1=res.to(cuda), pair=1, **kw)
-    e = rel_err(G.nchw(y2), want)
-    print(f"cta pair {B}x{H}x{W} {Cin}->{Cout} {kw}: rel err {e:.2e}, max |pair - single| {(y1 - y2).abs().max().item():.2e}")
-    assert e <= 2e-5
-    assert torch.equal(y1, y2), "same MMAs in the same order: the paired kernel must be bit-identical"
+    e1, e2 = rel_err(G.nchw(y1), want), rel_err(G.nchw(y2), want)
+    print(f"tile shapes {B}x{H}x{W} {Cin}->{Cout} {kw}: rel err {e1:.2e} / {e2:.2e}")
+    assert e1 <= 2e-5 and e2 <= 2e-5
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(1, 6, 128, 64, 64), (2, 5, 200, 64, 64), (1, 9, 384, 128, 128),
                                            (1, 4, 130, 256, 128), (2, 7, 256, 128, 64), (3, 40, 256, 128, 128),
-                                           # 64 -> 64: weights resident in smem; > 148 tiles so CTAs loop over several
+                                           # 64 -> 64 with > 132 tiles, so persistent CTAs loop over several
                                            (4, 48, 256, 64, 64)])
 def test_tc_strip_mode(cuda, B, H, W, Cin, Cout):
-    """Row-strip tiles: the three horizontal taps read one shared 130-pixel activation strip through descriptors
-    offset by kw rows."""
+    """Maps at least 128 pixels wide against fp64, with femasr_tc_args.strip both 0 and 1 (a schedule hint the sm_90a
+    kernel accepts and ignores; each call must still be right)."""
     x, w, b = rnd(B, Cin, H, W, seed=50), rnd(Cout, Cin, 3, 3, seed=51, scale=0.03), rnd(Cout, seed=52)
     want = F.conv2d(x.double(), w.double(), b.double(), padding=1)
     res = rnd(B, H, W, Cout, seed=53).to(cuda)
@@ -178,19 +178,9 @@ def test_tc_strip_mode(cuda, B, H, W, Cin, Cout):
     blob, bg = G.tc_pack(w.to(cuda)), b.to(cuda)
     y0 = G.tc_igemm(hi, lo, blob, bg, Cout, 3, res1=res, strip=0, pair=0)
     y1 = G.tc_igemm(hi, lo, blob, bg, Cout, 3, res1=res, strip=1)
-    e = rel_err(G.nchw(y1), want)
-    print(f"strip {B}x{H}x{W} {Cin}->{Cout}: rel err {e:.2e}, max |strip - per-tap| {(y0 - y1).abs().max().item():.2e}")
-    assert e <= 2e-5
-    # same products, different accumulation order (kh, chunk, kw instead of tap, chunk): equal up to accumulator rounding
-    assert (y0 - y1).abs().max().item() <= 1e-5 * y0.abs().max().item()
-    if Cout == 128:
-        # strips over a CTA pair (two neighbouring row tiles, each CTA stages half of every weight tile): same MMAs, same order
-        y2 = G.tc_igemm(hi, lo, blob, bg, Cout, 3, res1=res, strip=1, pair=1)
-        assert torch.equal(y1, y2), "the paired strip kernel must be bit-identical to the single-CTA one"
-        h8, x8 = G.tc_prepare_f8(G.nhwc(x).to(cuda))
-        b8 = G.tc_pack_f8(w.to(cuda))
-        assert torch.equal(G.tc_igemm(h8, x8, b8, bg, Cout, 3, res1=res, strip=1, pair=0, f8=1),
-                           G.tc_igemm(h8, x8, b8, bg, Cout, 3, res1=res, strip=1, pair=1, f8=1))
+    e0, e1 = rel_err(G.nchw(y0), want), rel_err(G.nchw(y1), want)
+    print(f"wide rows {B}x{H}x{W} {Cin}->{Cout}: rel err {e0:.2e} / {e1:.2e}")
+    assert e0 <= 2e-5 and e1 <= 2e-5
 
 
 def test_in_conv_split_planes(cuda):
@@ -326,9 +316,9 @@ def test_stage_taps_tensor_core_path(cuda):
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout,kw", [
-    (1, 24, 40, 256, 256, {}),                 # generic tiles, CTA pair
-    (1, 9, 384, 128, 128, {}),                 # row strips, streamed weights
-    (2, 10, 256, 64, 64, {}),                  # multi-row strips, resident weights
+    (1, 24, 40, 256, 256, {}),                 # 256 output channels: two 128-wide n-tiles
+    (1, 9, 384, 128, 128, {}),                 # wide rows
+    (2, 10, 256, 64, 64, {}),                  # 64-wide tiles
     (1, 12, 20, 256, 128, {"upsample": 1}),    # sub-pixel phase filters
     (2, 33, 17, 128, 64, {"pair": 0})])
 def test_tc_f8_cross_terms(cuda, B, H, W, Cin, Cout, kw):
