@@ -10,20 +10,40 @@ There is no CPU or eager-PyTorch fallback: calling the network without a CUDA sm
 In scope: norm_type 'gn', act_type 'silu'; one codebook at scale 32 or the multi-scale variant with further codebooks
 at 64 / 128 (femasr_arch.py:280-299); LQ_stage=True with scale_factor 2 or 4 (the SR network) and LQ_stage=False (the
 HQ autoencoder that produces gt_indices / codebook visualisations); the gt_indices loss value (femasr_arch.py:84-90);
+use_semantic_loss=True (the HQ-pretrain stage's VGG19 relu4_4 semantic loss, femasr_arch.py:301-309, 318-320, 344-347);
 inference only (no autograd through the engine).  Anything else raises NotImplementedError at construction instead of
 silently computing something different.
 """
 from __future__ import annotations
 
 import math
+import os
+import warnings
 
 import numpy as np
 import torch
 from torch import nn
 
 from basicsr.utils.registry import ARCH_REGISTRY
+from femasr_b200.lib import FemasrError
 from femasr_b200.net import NativeNet
-from femasr_b200.spec import normalize_codebooks, param_spec, relative_position_index, shift_attn_mask
+from femasr_b200.spec import (VGG_CONVS, VGG_TORCHVISION_INDEX, normalize_codebooks, param_spec, relative_position_index,
+                              shift_attn_mask, vgg_init)
+
+VGG_PRETRAIN_PATH = 'experiments/pretrained_models/vgg19-dcbb9e9d.pth'     # vgg_arch.py:9, relative to the working dir
+
+
+def _vgg_pretrained():
+    """The extractor's conv tensors from torchvision's vgg19 state_dict file (features.{0,2,5,...,25} -> conv1_1 ...
+    conv4_4) when it exists, like the reference (vgg_arch.py:104-107); else None.  Never downloads."""
+    if not os.path.exists(VGG_PRETRAIN_PATH):
+        return None
+    sd = torch.load(VGG_PRETRAIN_PATH, map_location="cpu")
+    out = {}
+    for (name, _ci, _co), i in zip(VGG_CONVS, VGG_TORCHVISION_INDEX):
+        for t in ("weight", "bias"):
+            out[f"vgg_feat_extractor.vgg_net.{name}.{t}"] = sd[f"features.{i}.{t}"].detach().float().clone()
+    return out
 
 
 class _Node(nn.Module):
@@ -83,8 +103,6 @@ class FeMaSRNet(nn.Module):
             unsupported.append(f"norm_type={norm_type!r}/act_type={act_type!r}")
         if (LQ_stage and scale_factor not in (2, 4)) or gt_resolution != 256 or in_channel != 3:
             unsupported.append("LQ-stage scale_factor not in {2,4} / gt_resolution != 256 / in_channel != 3")
-        if use_semantic_loss:
-            unsupported.append("use_semantic_loss=True (training-only VGG branch)")
         if unsupported:
             raise NotImplementedError("femasr_b200 implements the inference hot path only; unsupported: "
                                       + "; ".join(unsupported))
@@ -96,16 +114,31 @@ class FeMaSRNet(nn.Module):
         self.LQ_stage = LQ_stage
         self.scale_factor = scale_factor if LQ_stage else 1      # femasr_arch.py:241
         self.use_residual = use_residual
-        self.use_semantic_loss = False
+        self.use_semantic_loss = bool(use_semantic_loss)     # may be toggled like the reference's test() does (:451-452)
+        self._semantic_params = bool(use_semantic_loss)      # whether conv_semantic / vgg_feat_extractor exist
         self.max_depth = int(np.log2(gt_resolution // self.codebook_scale[0]))
         self.gemm_path = int(ignore_kwargs.get("gemm_path", -1))    # -1: engine default
 
+        vgg = None
+        if self._semantic_params:
+            vgg = _vgg_pretrained()
+            if vgg is None:
+                warnings.warn(f"use_semantic_loss: {VGG_PRETRAIN_PATH} not found; the VGG19 feature extractor is "
+                              "initialised randomly (torchvision's VGG init). ImageNet VGG19 weights are expected from a "
+                              "checkpoint; nothing is downloaded.", UserWarning, stacklevel=2)
         for name, shape, kind, fan_in in param_spec(self.scale_factor, self.e_dim, self.n_e, in_channel,
-                                                    codebooks=self.codebooks):
+                                                    codebooks=self.codebooks, semantic=self._semantic_params):
             if kind == "rpi":
                 _attach(self, name, relative_position_index(), buffer=True)
             elif kind == "mask":
                 _attach(self, name, shift_attn_mask(32, 32), buffer=True)
+            elif kind in ("vgg_mean", "vgg_std"):
+                _attach(self, name, vgg_init(shape, kind, fan_in), buffer=True)
+            elif kind in ("vgg_w", "vgg_b"):
+                t = vgg[name] if vgg is not None else vgg_init(shape, kind, fan_in)
+                if tuple(t.shape) != tuple(shape):
+                    raise ValueError(f"{VGG_PRETRAIN_PATH}: {name} has shape {tuple(t.shape)}, expected {tuple(shape)}")
+                _attach(self, name, t, buffer=False)
             else:
                 _attach(self, name, _init_tensor(shape, kind, fan_in, fan_in), buffer=False)   # codebook: fan_in = its n_e
         self._engine = None
@@ -151,7 +184,8 @@ class FeMaSRNet(nn.Module):
         if self._engine is None:
             gp = self.gemm_path if self.gemm_path >= 0 else default_gemm_path()
             self._engine = NativeNet(self.scale_factor, self.n_e, self.e_dim, self.use_quantize,
-                                     self.use_residual, gemm_path=gp, codebooks=self.codebooks)
+                                     self.use_residual, gemm_path=gp, codebooks=self.codebooks,
+                                     use_semantic_loss=self._semantic_params)
         if sig != self._engine_sig:
             self._engine.load_state_dict(dict(plist), device)
             self._engine_sig = sig
@@ -169,17 +203,24 @@ class FeMaSRNet(nn.Module):
     def encode_and_decode(self, input, gt_indices=None, current_iter=None):
         """femasr_arch.py:311-374 -> (out_img, codebook_loss, semantic_loss, [indices per codebook]).
         ``gt_indices`` (list, one map per codebook) switches codebook_loss to the supervised form (:84-90); the value
-        is computed, no autograd graph is attached."""
+        is computed, no autograd graph is attached.  semantic_loss is the VGG19 relu4_4 loss (:344-347, 372) while
+        ``use_semantic_loss`` is set, else codebook_loss * 0."""
+        want_sem = bool(self.use_semantic_loss)
+        if want_sem and not self._semantic_params:
+            raise FemasrError("use_semantic_loss was switched on for a network built without it "
+                              "(it has no conv_semantic / vgg_feat_extractor)")
         eng = self._native(input.device)
         if eng.use_graph and input.is_cuda and gt_indices is None and len(self.codebooks) == 1:
             # fixed launch list replayed as a CUDA graph; results are copied out of the graph's static buffers so the
             # returned tensors stay valid across calls like the reference's
-            out, loss, idx = eng.forward_graph(input)
+            res = eng.forward_graph(input, want_sem=want_sem)
             if eng.last_from_graph:
-                out, loss, idx = out.clone(), loss.clone(), idx.clone()
+                res = tuple(t.clone() for t in res)
         else:
-            out, loss, idx = eng.forward(input, gt_indices=gt_indices)
-        return out, loss, loss * 0, (idx if isinstance(idx, list) else [idx])
+            res = eng.forward(input, gt_indices=gt_indices, want_sem=want_sem)
+        out, loss, idx = res[:3]
+        sem = res[3] if want_sem else loss * 0
+        return out, loss, sem, (idx if isinstance(idx, list) else [idx])
 
     def decode_indices(self, indices):
         """femasr_arch.py:376-385."""

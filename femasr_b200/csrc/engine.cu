@@ -115,6 +115,8 @@ struct femasr_net {
   int tc_slice_kb = 4;                    // K-slice length in 64-wide k-blocks (FEMASR_TC_SLICE_KB; study knob)
   bool vq_fused = true;                   // VQ distances on the tensor cores with the argmin fused (FEMASR_VQ_FUSED=0: fp32 SIMT z.E^T + vq_select)
   bool fast_silu = true;                  // approximate-unit SiLU in the operand staging behind the VQ (FEMASR_FAST_SILU=0: exact)
+  bool semantic = false;                  // femasr_net_enable_semantic: the VGG19 / conv_semantic tensors are part of the spec
+  int sem_slice_kb = 0;                   // K-slice length of the semantic branch's GEMMs (FEMASR_SEM_SLICE_KB; study knob, 0 = one pass)
   std::vector<ProfRec> prof;
   std::string prof_json;
   ~femasr_net() {
@@ -201,12 +203,33 @@ static void build_spec(femasr_net* n) {
   }
 }
 
+// VGG19 features up to relu4_4 (vgg_arch.py:55-139 with layer_name_list ['relu4_4']): every conv is 3x3 pad 1 + ReLU,
+// a 2x2/2 max-pool sits in front of conv2_1, conv3_1 and conv4_1.
+static const char* const VGG_CONVS[12] = {"conv1_1", "conv1_2", "conv2_1", "conv2_2", "conv3_1", "conv3_2",
+                                          "conv3_3", "conv3_4", "conv4_1", "conv4_2", "conv4_3", "conv4_4"};
+static const int VGG_COUT[12] = {64, 64, 128, 128, 256, 256, 256, 256, 512, 512, 512, 512};
+static const bool VGG_POOL_BEFORE[12] = {false, false, true, false, true, false, false, false, true, false, false, false};
+
+// use_semantic_loss=True (femasr_arch.py:301-309): conv_semantic = Sequential(Conv2d(512, 512, 1), ReLU) and the extractor
+static void add_semantic(femasr_net* n) {
+  add_conv(n, "conv_semantic.0", 512, 512, 1);
+  add_vec(n, "vgg_feat_extractor.mean", 3);
+  add_vec(n, "vgg_feat_extractor.std", 3);
+  int cin = 3;
+  for (int i = 0; i < 12; ++i) {
+    add_conv(n, std::string("vgg_feat_extractor.vgg_net.") + VGG_CONVS[i], cin, VGG_COUT[i], 3);
+    cin = VGG_COUT[i];
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 struct Ctx {
   femasr_net* net;
   Arena ar;
   cudaStream_t st;
   int status = FEMASR_OK;
+  float* sem_loss = nullptr;     // forward_sem: the semantic loss output (non-NULL = run the VGG branch)
+  float* vgg_feat = nullptr;     // relu4_4 [B,H/8,W/8,512], alive from the VGG stage to the loss at quantising level 0
   bool precise_region = false;   // true while emitting the layers in front of the VQ (index-critical)
   bool dry() const { return ar.dry; }
   bool ok() const { return status == FEMASR_OK; }
@@ -485,6 +508,111 @@ struct Ctx {
     ar.release(rs); ar.release(mu); ar.release(hid); ar.release(ao); ar.release(qkv); ar.release(T);
   }
 
+  // One GEMM of the semantic branch with the ReLU epilogue (bias, then ReLU): the 3-product split-fp16 wgmma GEMM in one
+  // pass (no K slices, no F8) on gemm_path 1, the fp32 SIMT GEMM on gemm_path 0.  wkey: the packed weight's key.
+  void sem_gemm(const char* name, const std::string& wname, const std::string& wkey, const void* ahi, const void* alo,
+                const float* ax, float* y, void* ohi, void* olo, int B, int H, int W, int Cin, int Cout, int ksize,
+                double flops) {
+    if (dry() || !ok()) return;
+    if (net->cfg.gemm_path == 1) {
+      auto it = net->tcw.find(wkey);
+      if (it == net->tcw.end()) { check(fail(FEMASR_ERR_STATE, "parameter not set: " + wname + ".weight")); return; }
+      femasr_tc_args t;
+      memset(&t, 0, sizeof(t));
+      t.a_hi = ahi; t.a_lo = alo; t.w_blob = it->second.p; t.bias = P(wname + ".bias");
+      t.y = y; t.out_hi = ohi; t.out_lo = olo;
+      t.B = B; t.H = H; t.W = W; t.Cin = Cin; t.Cout = Cout; t.ksize = ksize; t.act = FEMASR_ACT_RELU;
+      t.stride = 1; t.pair = -1; t.strip = -1; t.slice_kb = net->sem_slice_kb;
+      run(name, flops, [&] { return femasr_tc_igemm(&t, st); });
+    } else {
+      femasr_igemm_args a;
+      memset(&a, 0, sizeof(a));
+      a.x = ax; a.w = P(wkey); a.bias = P(wname + ".bias"); a.y = y;
+      a.B = B; a.Hin = H; a.Win = W; a.Cin = Cin; a.Cout = Cout; a.ksize = ksize; a.stride = 1; a.act = FEMASR_ACT_RELU;
+      if (!ok()) return;
+      run(name, flops, [&] { return femasr_igemm_simt(&a, st); });
+    }
+  }
+
+  // vgg_feat = relu4_4((x - mean) / std) (femasr_arch.py:318-320).  Runs before the encoder: relu4_4 is allocated first
+  // and every full-resolution VGG buffer is released before the encoder's peak.  gemm_path 1 hands the activations from
+  // conv to conv as split fp16 planes; the pools read fp32 (pooling before the split) and write the next conv's planes.
+  void semantic_vgg(const float* x_nchw, int B, int H, int W) {
+    const bool tc = net->cfg.gemm_path == 1;
+    const std::string pre = "vgg_feat_extractor.vgg_net.";
+    vgg_feat = ar.alloc((size_t)B * (H / 8) * (W / 8) * 512);
+    int h = H, w = W, c = 64;
+    float *ahi = nullptr, *alo = nullptr, *af = nullptr;   // the current conv's operand: split planes (tc) or fp32
+    {
+      const size_t rows = (size_t)B * H * W;
+      if (tc) { ahi = ar.alloc(rows * 32); alo = ar.alloc(rows * 32); } else { af = ar.alloc(rows * 64); }
+      const float *mean = P("vgg_feat_extractor.mean"), *sd = P("vgg_feat_extractor.std");
+      run("vgg_im2col", 0.0, [&] { return femasr_vgg_im2col(x_nchw, mean, sd, ahi, alo, af, B, H, W, st); });
+    }
+    float* f = nullptr;                                    // fp32 output in front of a pool
+    for (int i = 0; i < 12; ++i) {
+      const int co = VGG_COUT[i];
+      if (VGG_POOL_BEFORE[i]) {
+        const size_t n2 = (size_t)B * (h / 2) * (w / 2) * c;
+        if (tc) {
+          ahi = ar.alloc((n2 + 1) / 2); alo = ar.alloc((n2 + 1) / 2);
+          const int hh = h, ww = w, cc = c;
+          run("vgg_pool", 0.0, [&] {
+            return femasr_tc_prepare(f, ahi, alo, FEMASR_PRO_MAXPOOL2, nullptr, nullptr, nullptr, nullptr, B, hh, ww, cc, 0, 0.f, st);
+          });
+        } else {
+          af = ar.alloc(n2);
+          const int hh = h, ww = w, cc = c;
+          run("vgg_pool", 0.0, [&] { return femasr_maxpool2(f, af, B, hh, ww, cc, st); });
+        }
+        ar.release(f); f = nullptr;
+        h /= 2; w /= 2;
+      }
+      const bool last = i == 11, to_f32 = !tc || last || VGG_POOL_BEFORE[i + 1];
+      const size_t n = (size_t)B * h * w * co;
+      float* y = last ? vgg_feat : (to_f32 ? ar.alloc(n) : nullptr);
+      float *ohi = nullptr, *olo = nullptr;
+      if (!to_f32) { ohi = ar.alloc((n + 1) / 2); olo = ar.alloc((n + 1) / 2); }
+      const std::string wn = pre + VGG_CONVS[i];
+      const double flops = 2.0 * B * h * (double)w * co * (i == 0 ? 27 : 9 * c);   // algorithmic (27 MACs for conv1_1)
+      if (i == 0)       // conv1_1: 1x1 GEMM over the K = 27 -> 64 im2col rows
+        sem_gemm("vgg_conv", wn, wn + ".weight#im2col", ahi, alo, af, y, ohi, olo, B, h, w, 64, co, 1, flops);
+      else
+        sem_gemm("vgg_conv", wn, wn + ".weight", ahi, alo, af, y, ohi, olo, B, h, w, c, co, 3, flops);
+      if (tc) { ar.release(alo); ar.release(ahi); ahi = ohi; alo = olo; }
+      else { ar.release(af); af = y; }
+      if (to_f32 && !last) f = y;
+      c = co;
+    }
+    tap("vgg", vgg_feat, (size_t)B * h * w * 512);
+  }
+
+  // semantic_loss = mse(ReLU(conv_semantic(z_quant)), vgg_feat) (femasr_arch.py:344-347) on the quantiser's output
+  // (before the use_quantize override, :349-350); the only quantising level where the shapes agree is level 0 of the HQ
+  // stage, so the sum over levels (:372) is this one term.
+  void semantic_loss(const float* zq, int B, int hh, int ww) {
+    const size_t N = (size_t)B * hh * ww;
+    const bool tc = net->cfg.gemm_path == 1;
+    float* s = ar.alloc(N * 512);
+    float* rows = ar.alloc(N);
+    float *zhi = nullptr, *zlo = nullptr;
+    if (tc) {
+      zhi = ar.alloc(N * 256); zlo = ar.alloc(N * 256);
+      run("tc_prepare", 0.0, [&] { return femasr_tc_prepare(zq, zhi, zlo, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, B, hh, ww, 512, 0, 0.f, st); });
+    }
+    sem_gemm("semantic_conv", "conv_semantic.0", "conv_semantic.0.weight", zhi, zlo, zq, s, nullptr, nullptr, B, hh, ww,
+             512, 512, 1, 2.0 * N * 512 * 512);
+    tap("semantic", s, N * 512);
+    if (!dry() && ok()) {
+      const float* v = vgg_feat;
+      run("semantic_mse", 0.0, [&] { return femasr_sq_diff_rows(s, v, rows, (int)N, 512, st); });
+      run("semantic_mse", 0.0, [&] { return femasr_sum_scaled(rows, sem_loss, N, 1.0 / ((double)N * 512), st); });
+    }
+    if (tc) { ar.release(zlo); ar.release(zhi); }
+    ar.release(rows); ar.release(s);
+    ar.release(vgg_feat); vgg_feat = nullptr;
+  }
+
   // One quantiser (femasr_arch.py:337-342 + VectorQuantizer.forward :50-100): z = before_quant(src) [N,e], argmin over
   // codebook k, zq = z + (E[idx] - z); loss terms accumulate into cb_loss.  Returns z and zq (caller releases both).
   void quantise(int k, const float* src, int Cin, int B, int hh, int ww, int64_t* indices, float* cb_loss,
@@ -580,6 +708,7 @@ struct Ctx {
           }
           quantise(k, src, Cin, B, hh, ww, indices ? indices + idx_off : nullptr, cb_loss,
                    gt ? gt + idx_off : nullptr, &z, &zq);
+          if (k == 0 && sem_loss) semantic_loss(zq, B, hh, ww);
           idx_off += N;
           if (cat) ar.release(cat);
           aq = cfg.use_quantize ? zq : z;     // :349-350
@@ -633,6 +762,7 @@ struct Ctx {
     int c = chan(256 / cfg.scale_factor);
     int h = H - 1, w = W - 1;
     const bool tc = tc_convs(c);
+    if (sem_loss) semantic_vgg(x_nchw, B, H, W);
     precise_region = true;
     const float *iw = P(enc + ".in_conv.weight"), *ib = P(enc + ".in_conv.bias");
     const double in_flops = 2.0 * 16 * cfg.in_channel * c * (double)B * h * w;
@@ -746,6 +876,38 @@ static int check_geometry(femasr_net* net, int B, int H, int W) {
   return FEMASR_OK;
 }
 
+// the semantic loss exists where ReLU(conv_semantic(z_quant)) [B,512,h,w] meets relu4_4 [B,512,H/8,W/8] at every
+// quantising level; elsewhere the reference raises from conv_semantic (channels) or mse_loss (sizes)
+static int check_semantic(femasr_net* net, int H, int W) {
+  if (!net->semantic) return fail(FEMASR_ERR_STATE, "forward_sem: the net was created without femasr_net_enable_semantic");
+  const int div = net->hq ? 8 : (net->cfg.scale_factor == 4 ? 2 : 4);
+  const std::string vgg = "relu4_4 is [B,512," + std::to_string(H / 8) + "," + std::to_string(W / 8) + "]";
+  for (size_t k = 0; k < net->cbs.size(); ++k) {
+    const femasr_net::Codebook& cb = net->cbs[k];
+    const int m = cb.scale / 32, zh = H / div * m, zw = W / div * m;
+    const std::string z = "[B," + std::to_string(cb.e_dim) + "," + std::to_string(zh) + "," + std::to_string(zw) + "]";
+    if (cb.e_dim != 512)
+      return fail(FEMASR_ERR_ARG, "semantic loss: conv_semantic takes 512 channels but z_quant of codebook " +
+                                      std::to_string(k) + " is " + z + "; " + vgg);
+    if (zh != H / 8 || zw != W / 8)
+      return fail(FEMASR_ERR_ARG, "semantic loss: ReLU(conv_semantic(z_quant)) of codebook " + std::to_string(k) + " is " + z +
+                                      " but " + vgg);
+  }
+  return FEMASR_OK;
+}
+
+static int workspace_impl(femasr_net* net, int B, int H, int W, bool with_sem, size_t* bytes) {
+  int s = check_geometry(net, B, H, W);
+  if (s) return s;
+  if (with_sem && (s = check_semantic(net, H, W))) return s;
+  Ctx c; c.net = net; c.st = nullptr; c.ar.dry = true; c.ar.base = reinterpret_cast<char*>(uintptr_t(1) << 40);
+  if (with_sem) c.sem_loss = reinterpret_cast<float*>(uintptr_t(8));
+  // sized for the gt_indices loss branch too (its scratch is small): one workspace serves forward and forward_gt
+  c.forward(nullptr, nullptr, nullptr, nullptr, reinterpret_cast<const int64_t*>(uintptr_t(8)), B, H, W);
+  *bytes = c.ar.peak + 256;
+  return c.status;
+}
+
 }  // namespace femasr
 
 extern "C" const char* femasr_last_error(void) { return g_err.c_str(); }
@@ -796,12 +958,22 @@ extern "C" int femasr_net_create(const femasr_net_config* cfg, femasr_net** out)
   if (const char* ev = getenv("FEMASR_IN_CONV_TC")) n->in_conv_tc = atoi(ev) != 0;
   if (const char* ev = getenv("FEMASR_F8_CROSS")) n->f8_cross = atoi(ev) != 0;
   if (const char* ev = getenv("FEMASR_TC_SLICE_KB")) n->tc_slice_kb = std::max(1, atoi(ev));
+  if (const char* ev = getenv("FEMASR_SEM_SLICE_KB")) n->sem_slice_kb = std::max(0, atoi(ev));
   build_spec(n);
   *out = n;
   return FEMASR_OK;
 }
 
 extern "C" void femasr_net_destroy(femasr_net* net) { delete net; }
+
+extern "C" int femasr_net_enable_semantic(femasr_net* net) {
+  FEMASR_CHECK_ARG(net, "enable_semantic: null");
+  if (net->semantic) return FEMASR_OK;
+  if (!net->raw.empty()) return fail(FEMASR_ERR_STATE, "enable_semantic: call it before the first set_param");
+  add_semantic(net);
+  net->semantic = true;
+  return FEMASR_OK;
+}
 
 extern "C" int femasr_net_set_param(femasr_net* net, const char* name, const float* data, size_t numel, int on_device,
                                     void* stream) {
@@ -821,6 +993,26 @@ extern "C" int femasr_net_set_param(femasr_net* net, const char* name, const flo
     if (!pb.p) { FEMASR_CUDA(cudaMalloc(&pb.p, numel * sizeof(float))); pb.n = numel; }
     int s = femasr_pack_weight(rb.p, pb.p, pi.Cout, pi.Cin, pi.k, pi.k, st);
     if (s) return s;
+    const bool vgg = key.rfind("vgg_feat_extractor.", 0) == 0;
+    if (vgg && pi.Cin == 3) {
+      // VGG conv1_1 as a K = 27 -> 64 GEMM over normalised im2col rows: [Cout][64] padded matrix -> K-major fp32
+      // (gemm_path 0) or split-fp16 blob (gemm_path 1)
+      float* tmp = nullptr;
+      FEMASR_CUDA(cudaMallocAsync(&tmp, (size_t)pi.Cout * 64 * sizeof(float), st));
+      s = femasr_vgg_pad_weight(rb.p, tmp, pi.Cout, st);
+      if (!s && net->cfg.gemm_path == 1) {
+        DevBuf& tb = net->tcw[key + "#im2col"];
+        const size_t bytes = femasr_tc_weight_bytes(pi.Cout, 64, 1, 1);
+        if (!tb.p) { if (cudaMalloc(&tb.p, bytes) != cudaSuccess) s = fail(FEMASR_ERR_CUDA, "cudaMalloc failed"); tb.n = bytes / sizeof(float); }
+        if (!s) s = femasr_tc_pack_weight(tmp, tb.p, pi.Cout, 64, 1, 1, st);
+      } else if (!s) {
+        DevBuf& kb = net->packed[key + "#im2col"];
+        if (!kb.p) { if (cudaMalloc(&kb.p, (size_t)pi.Cout * 64 * sizeof(float)) != cudaSuccess) s = fail(FEMASR_ERR_CUDA, "cudaMalloc failed"); kb.n = (size_t)pi.Cout * 64; }
+        if (!s) s = femasr_pack_weight(tmp, kb.p, pi.Cout, 64, 1, 1, st);
+      }
+      cudaFreeAsync(tmp, st);
+      return s;
+    }
     if (net->cfg.gemm_path == 1 && net->in_conv_tc && pi.k == 4 && pi.Cin == 3 && pi.Cout % 64 == 0) {
       // in_conv as a K = 48 -> 64 tensor-core GEMM over im2col rows: [Cout][64] padded matrix -> split-fp16 blob
       float* tmp = nullptr;
@@ -839,7 +1031,7 @@ extern "C" int femasr_net_set_param(femasr_net* net, const char* name, const flo
       if (!tb.p) { FEMASR_CUDA(cudaMalloc(&tb.p, bytes)); tb.n = bytes / sizeof(float); }
       s = femasr_tc_pack_weight(rb.p, tb.p, pi.Cout, pi.Cin, pi.k, pi.k, st);
       if (s) return s;
-      if (net->f8_cross && pi.k == 3) {      // a 3x3 conv may run behind the VQ: keep the F8 packing next to the fp16 one
+      if (net->f8_cross && pi.k == 3 && !vgg) {      // a 3x3 conv may run behind the VQ (the VGG convs never use F8): keep the F8 packing next to the fp16 one
         DevBuf& t8 = net->tcw8[key];
         if (!t8.p) { FEMASR_CUDA(cudaMalloc(&t8.p, bytes)); t8.n = bytes / sizeof(float); }
         s = femasr_tc_pack_weight_f8(rb.p, t8.p, pi.Cout, pi.Cin, pi.k, pi.k, st);
@@ -902,13 +1094,12 @@ extern "C" int femasr_net_params_complete(femasr_net* net) {
 
 extern "C" int femasr_net_workspace_bytes(femasr_net* net, int B, int H, int W, size_t* bytes) {
   FEMASR_CHECK_ARG(net && bytes, "workspace_bytes: null pointer");
-  int s = check_geometry(net, B, H, W);
-  if (s) return s;
-  Ctx c; c.net = net; c.st = nullptr; c.ar.dry = true; c.ar.base = reinterpret_cast<char*>(uintptr_t(1) << 40);
-  // sized for the gt_indices loss branch too (its scratch is small): one workspace serves forward and forward_gt
-  c.forward(nullptr, nullptr, nullptr, nullptr, reinterpret_cast<const int64_t*>(uintptr_t(8)), B, H, W);
-  *bytes = c.ar.peak + 256;
-  return c.status;
+  return workspace_impl(net, B, H, W, false, bytes);
+}
+
+extern "C" int femasr_net_workspace_bytes_sem(femasr_net* net, int B, int H, int W, int with_sem, size_t* bytes) {
+  FEMASR_CHECK_ARG(net && bytes, "workspace_bytes_sem: null pointer");
+  return workspace_impl(net, B, H, W, with_sem != 0, bytes);
 }
 
 extern "C" int femasr_net_forward(femasr_net* net, const float* x, float* y, int64_t* indices, float* cb_loss, int B,
@@ -919,17 +1110,23 @@ extern "C" int femasr_net_forward(femasr_net* net, const float* x, float* y, int
 extern "C" int femasr_net_forward_gt(femasr_net* net, const float* x, float* y, int64_t* indices, float* cb_loss,
                                      const int64_t* gt_indices, int B, int H, int W, void* workspace,
                                      size_t workspace_bytes, void* stream) {
+  return femasr_net_forward_sem(net, x, y, indices, cb_loss, gt_indices, nullptr, B, H, W, workspace, workspace_bytes, stream);
+}
+
+extern "C" int femasr_net_forward_sem(femasr_net* net, const float* x, float* y, int64_t* indices, float* cb_loss,
+                                      const int64_t* gt_indices, float* sem_loss, int B, int H, int W, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
   FEMASR_CHECK_ARG(net && x && y && workspace, "forward: null pointer");
   int s = check_geometry(net, B, H, W);
   if (s) return s;
   s = femasr_net_params_complete(net);
   if (s) return s;
   size_t need = 0;
-  s = femasr_net_workspace_bytes(net, B, H, W, &need);
+  s = workspace_impl(net, B, H, W, sem_loss != nullptr, &need);
   if (s) return s;
   const uintptr_t mis = (256 - ((uintptr_t)workspace & 255)) & 255;
   if (workspace_bytes < need) return fail(FEMASR_ERR_STATE, "forward: workspace too small (need " + std::to_string(need) + " bytes)");
-  Ctx c; c.net = net; c.st = as_stream(stream); c.ar.dry = false;
+  Ctx c; c.net = net; c.st = as_stream(stream); c.ar.dry = false; c.sem_loss = sem_loss;
   c.ar.base = reinterpret_cast<char*>(workspace) + mis; c.ar.cap = workspace_bytes - mis;
   const long l0 = g_launches;
   c.forward(x, y, indices, cb_loss, gt_indices, B, H, W);
@@ -965,7 +1162,8 @@ extern "C" int femasr_net_decode_indices(femasr_net* net, const int64_t* indices
 
 extern "C" int femasr_net_set_tap(femasr_net* net, const char* stage, float* dst, size_t capacity) {
   FEMASR_CHECK_ARG(net && stage, "set_tap: null pointer");
-  static const char* names[] = {"in_conv", "down", "swin", "up1", "up2", "z", "zq", "after_quant", "dec0", "dec1", "dec2", "z1", "z2"};
+  static const char* names[] = {"in_conv", "down", "swin", "up1", "up2", "z", "zq", "after_quant", "dec0", "dec1", "dec2", "z1", "z2",
+                                "vgg", "semantic"};
   bool known = false;
   for (const char* n : names) known = known || strcmp(n, stage) == 0;
   if (!known) return fail(FEMASR_ERR_ARG, std::string("set_tap: unknown stage ") + stage);

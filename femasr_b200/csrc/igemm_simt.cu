@@ -151,6 +151,7 @@ __global__ void __launch_bounds__(256, 2) igemm_simt_kernel(const IgemmP p) {
         o.x += bv.x; o.y += bv.y; o.z += bv.z; o.w += bv.w;
       }
       if (p.act == FEMASR_ACT_GELU) { o.x = gelu_erf_f(o.x); o.y = gelu_erf_f(o.y); o.z = gelu_erf_f(o.z); o.w = gelu_erf_f(o.w); }
+      else if (p.act == FEMASR_ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
       const long off = m * p.Cout + n;
       if (p.res1) {
         const float4 r = *reinterpret_cast<const float4*>(p.res1 + off);

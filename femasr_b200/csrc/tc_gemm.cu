@@ -406,7 +406,7 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
       continue;
     }
 
-    // ===================== epilogue: acc * 2^-s + bias -> GELU -> + res1 + res2 -> store =====================
+    // ===================== epilogue: acc * 2^-s + bias -> GELU | ReLU -> + res1 + res2 -> store =====================
     const int Ho = p.up ? 2 * p.H : p.H, Wo = p.up ? 2 * p.W : p.W;
     long off[2];                                         // output element offset of this thread's two rows (-1: outside)
 #pragma unroll
@@ -428,6 +428,7 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
         o.x = fmaf(acc[4 * j + 2 * h], inv_scale, bb.x);     // acc * 2^-s is exact: == (acc * inv) + bias
         o.y = fmaf(acc[4 * j + 2 * h + 1], inv_scale, bb.y);
         if (p.act == FEMASR_ACT_GELU) { o.x = gelu_erf_fast_f(o.x); o.y = gelu_erf_fast_f(o.y); }
+        else if (p.act == FEMASR_ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
         if (off[h] >= 0) {
           const long o_off = off[h] + col;
           if (RES) { const float2 r = *reinterpret_cast<const float2*>(p.res1 + o_off); o.x += r.x; o.y += r.y; }
@@ -525,6 +526,17 @@ __global__ void __launch_bounds__(256) tc_prepare_kernel(const float* __restrict
         split_store8(v, hi + op, lo + op);
       }
   }
+}
+
+// nn.MaxPool2d(2, 2) (floor) fused into the staging of the next conv's operand: the max is taken on fp32 and then split,
+// so the planes are exactly the split of the pooled tensor.  x [B,H,W,C] -> [B,H/2,W/2,C], 8 channels per thread.
+__global__ void __launch_bounds__(256) tc_prepare_pool_kernel(const float* __restrict__ x, __half* __restrict__ hi,
+                                                              __half* __restrict__ lo, int H, int W, int C, long total8) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total8) return;
+  float v[8];
+  const long o = pool2_max8(x, i, H, W, C, v);
+  split_store8(v, hi + o, lo + o);
 }
 
 // Same transform without replication, organised for bandwidth: the image is a flat array of float4 (4 channels), a warp
@@ -985,6 +997,12 @@ extern "C" int femasr_tc_prepare(const float* x, void* a_hi, void* a_lo, int mod
     const long M = (long)B * H * W;
     FEMASR_CUDA(launch_pdl(tc_prepare_ln_kernel, dim3((unsigned)cdiv(M, 16)), dim3(256), 0, st, x, hi, lo, gamma, beta, M, eps));
     return launch_status("tc_prepare_ln_kernel");
+  }
+  if (mode == FEMASR_PRO_MAXPOOL2) {
+    FEMASR_CHECK_ARG(!upsample && H >= 2 && W >= 2, "tc_prepare: max-pool mode needs H, W >= 2 and no upsample");
+    const long total8 = (long)B * (H / 2) * (W / 2) * (C / 8);
+    tc_prepare_pool_kernel<<<(unsigned)cdiv(total8, 256), 256, 0, st>>>(x, hi, lo, H, W, C, total8);
+    return launch_status("tc_prepare_pool_kernel");
   }
   static const int flat_env = [] { const char* e = getenv("FEMASR_PREP_FLAT"); return e ? atoi(e) : 1; }();
   if (!upsample && flat_env && (long)H * W * (C / 4) < (1l << 30) && B <= 65535 &&

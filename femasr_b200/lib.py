@@ -11,10 +11,11 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("FEMASR_LIB") or os.path.join(_HERE, "libfemasr_b200.so")
 
-PRO_NONE, PRO_GN_SILU, PRO_LN, PRO_GN_SILU_FAST = 0, 1, 2, 3
+PRO_NONE, PRO_GN_SILU, PRO_LN, PRO_GN_SILU_FAST, PRO_MAXPOOL2 = 0, 1, 2, 3, 4
 ABI_VERSION = 4          # femasr_abi_version() of the library this binding was written against (include/femasr_b200.h)
-ACT_NONE, ACT_GELU = 0, 1
+ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
 TAP_STAGES = ("in_conv", "down", "swin", "up1", "up2", "z", "zq", "after_quant", "dec0", "dec1", "dec2")
+SEMANTIC_TAP_STAGES = ("vgg", "semantic")      # only in a forward that computes the semantic loss
 
 c_float_p = C.c_void_p     # raw device/host addresses travel as integers
 c_i64_p = C.c_void_p
@@ -63,6 +64,9 @@ SIGNATURES = {
     "femasr_net_set_param": (_I, [_V, C.c_char_p, _V, _Z, _I, _V]),
     "femasr_net_params_complete": (_I, [_V]),
     "femasr_net_workspace_bytes": (_I, [_V, _I, _I, _I, C.POINTER(_Z)]),
+    "femasr_net_enable_semantic": (_I, [_V]),
+    "femasr_net_workspace_bytes_sem": (_I, [_V, _I, _I, _I, _I, C.POINTER(_Z)]),
+    "femasr_net_forward_sem": (_I, [_V, _V, _V, _V, _V, _V, _V, _I, _I, _I, _V, _Z, _V]),
     "femasr_net_forward": (_I, [_V, _V, _V, _V, _V, _I, _I, _I, _V, _Z, _V]),
     "femasr_net_forward_gt": (_I, [_V, _V, _V, _V, _V, _V, _I, _I, _I, _V, _Z, _V]),
     "femasr_net_decode_indices": (_I, [_V, _V, _V, _I, _I, _I, _V, _Z, _V]),
@@ -113,6 +117,10 @@ SIGNATURES = {
     "femasr_in_conv4x4_split": (_I, [_V, _V, _V, _V, _V, _I, _I, _I, _I, _I, _V]),
     "femasr_in_conv_im2col": (_I, [_V, _V, _V, _I, _I, _I, _I, _V]),
     "femasr_in_conv_pad_weight": (_I, [_V, _V, _I, _V]),
+    "femasr_vgg_im2col": (_I, [_V, _V, _V, _V, _V, _V, _I, _I, _I, _V]),
+    "femasr_vgg_pad_weight": (_I, [_V, _V, _I, _V]),
+    "femasr_maxpool2": (_I, [_V, _V, _I, _I, _I, _I, _V]),
+    "femasr_sq_diff_rows": (_I, [_V, _V, _V, _I, _I, _V]),
     "femasr_out_conv3x3": (_I, [_V, _V, _V, _V, _I, _I, _I, _I, _V]),
     "femasr_out_conv3x3_mma": (_I, [_V, _V, _V, _V, _I, _I, _I, _I, _V]),
     "femasr_nchw_to_nhwc": (_I, [_V, _V, _I, _I, _I, _I, _V]),

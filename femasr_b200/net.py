@@ -50,9 +50,11 @@ def padded_size(n: int, scale: int) -> int:
 
 class NativeNet:
     def __init__(self, scale_factor: int, n_e: int, e_dim: int, use_quantize: bool = True,
-                 use_residual: bool = True, gemm_path: int = 0, codebooks=None):
+                 use_residual: bool = True, gemm_path: int = 0, codebooks=None, use_semantic_loss: bool = False):
         """``codebooks``: the reference's ``codebook_params`` rows [[scale, n_e, e_dim], ...] for the multi-scale
-        variant (femasr_arch.py:231-235); default one codebook (32, n_e, e_dim)."""
+        variant (femasr_arch.py:231-235); default one codebook (32, n_e, e_dim).  ``use_semantic_loss``: the engine also
+        holds the VGG19 / conv_semantic tensors (femasr_arch.py:301-309) and forward(want_sem=True) computes the HQ
+        stage's semantic loss."""
         self.lib = L.load()
         self.scale = int(scale_factor)
         self.codebooks = normalize_codebooks(codebooks, n_e, e_dim)
@@ -66,7 +68,9 @@ class NativeNet:
         self._ws: Optional[torch.Tensor] = None
         self._taps: Dict[str, torch.Tensor] = {}
         self.device: Optional[torch.device] = None
-        self.names = [n for (n, _s, kind, _f) in param_spec(self.scale, self.e_dim, self.n_e, codebooks=self.codebooks)
+        self.use_semantic_loss = bool(use_semantic_loss)
+        self.names = [n for (n, _s, kind, _f) in param_spec(self.scale, self.e_dim, self.n_e, codebooks=self.codebooks,
+                                                             semantic=self.use_semantic_loss)
                       if kind not in ("rpi", "mask")]
         # the forward is a fixed launch list per input shape: replay it as a CUDA graph (no per-launch host work)
         self.use_graph = os.environ.get("FEMASR_CUDA_GRAPH", "1") != "0"
@@ -87,6 +91,8 @@ class NativeNet:
             with torch.cuda.device(device):
                 L.require_device()
                 L.check(self.lib.femasr_net_create(C.byref(self.cfg), C.byref(self._h)))
+                if self.use_semantic_loss:
+                    L.check(self.lib.femasr_net_enable_semantic(self._h))
             self.device = device
         elif device != self.device:
             raise L.FemasrError(f"engine lives on {self.device}, input is on {device}")
@@ -139,11 +145,12 @@ class NativeNet:
         return [(B, 1, h * cs // 32, w * cs // 32) for cs, _n, _e in self.codebooks]
 
     def forward(self, x: torch.Tensor, want_indices: bool = True, want_loss: bool = True,
-                taps: Optional[List[str]] = None, gt_indices=None):
+                taps: Optional[List[str]] = None, gt_indices=None, want_sem: bool = False):
         """encode_and_decode.  x [B,3,H,W] fp32 cuda -> (y [B,3,sH,sW], loss scalar tensor | None,
-        indices [B,1,h,w] int64 | None[, {stage: NHWC tensor}]); multi-scale nets return a list of index maps, one
+        indices [B,1,h,w] int64 | None[, sem][, {stage: NHWC tensor}]); multi-scale nets return a list of index maps, one
         per codebook.  ``gt_indices`` (tensor or list, one map per codebook) selects the supervised loss of
-        femasr_arch.py:84-90 (LQ stage)."""
+        femasr_arch.py:84-90 (LQ stage).  ``want_sem``: also the semantic loss (scalar tensor, femasr_arch.py:344-347,
+        372), returned after the indices; needs use_semantic_loss and the HQ stage with one codebook of e_dim 512."""
         if x.dim() != 4 or x.shape[1] != 3:
             raise L.FemasrError(f"expected input [B,3,H,W], got {tuple(x.shape)}")
         self._ensure(x.device)
@@ -173,6 +180,9 @@ class NativeNet:
                     self._check_index_range(g_, ne_, "forward(gt_indices)")
                 gt = torch.cat([g.detach().to(self.device, torch.int64).reshape(-1) for g in gl]).contiguous()
             loss = torch.empty((), dtype=torch.float32, device=self.device) if want_loss else None
+            if want_sem and not self.use_semantic_loss:
+                raise L.FemasrError("the semantic loss needs an engine built with use_semantic_loss=True")
+            sem = torch.empty((), dtype=torch.float32, device=self.device) if want_sem else None
             tap_out = {}
             if taps:
                 shapes = self.tap_shapes(B, H, W)
@@ -182,26 +192,29 @@ class NativeNet:
                     L.check(self.lib.femasr_net_set_tap(self._h, name.encode(), t.data_ptr(), t.numel()))
             # sized AFTER the taps are registered: the engine's plan (and so its workspace) depends on them
             need = C.c_size_t()
-            L.check(self.lib.femasr_net_workspace_bytes(self._h, B, H, W, C.byref(need)))
-            ws = self._workspace(need.value)
             try:
-                L.check(self.lib.femasr_net_forward_gt(self._h, x.data_ptr(), y.data_ptr(), _ptr(flat), _ptr(loss),
-                                                       _ptr(gt), B, H, W, ws.data_ptr(), ws.numel(), _stream()))
+                L.check(self.lib.femasr_net_workspace_bytes_sem(self._h, B, H, W, int(want_sem), C.byref(need)))
+                ws = self._workspace(need.value)
+                L.check(self.lib.femasr_net_forward_sem(self._h, x.data_ptr(), y.data_ptr(), _ptr(flat), _ptr(loss),
+                                                        _ptr(gt), _ptr(sem), B, H, W, ws.data_ptr(), ws.numel(),
+                                                        _stream()))
             finally:
                 for name in tap_out:
                     self.lib.femasr_net_set_tap(self._h, name.encode(), None, 0)
+        res = (y, loss, idx) + ((sem,) if want_sem else ())
         if taps:
-            return y, loss, idx, tap_out
-        return y, loss, idx
+            return res + (tap_out,)
+        return res
 
-    def forward_graph(self, x: torch.Tensor):
-        """encode_and_decode through a captured CUDA graph.  Returns (y, loss, idx); when they come out of a graph
-        they live in its static output buffers: valid until the next call with the same shape (clone to keep).
+    def forward_graph(self, x: torch.Tensor, want_sem: bool = False):
+        """encode_and_decode through a captured CUDA graph.  Returns (y, loss, idx), with ``want_sem`` (y, loss, idx, sem);
+        when they come out of a graph they live in its static output buffers: valid until the next call with the same
+        shape (clone to keep).
         Policy: the first sighting of a shape runs eagerly (shared workspace); the second captures; at most
         ``graph_cache_size`` graphs are kept (least recently used evicted, its workspace and buffers freed)."""
         self._ensure(x.device)
         x = x.detach().float().contiguous()
-        key = tuple(x.shape)
+        key = tuple(x.shape) + (("sem",) if want_sem else ())
         ent = self._graphs.get(key)
         if ent is None:
             seen = self._seen_shapes.pop(key, 0) + 1
@@ -210,7 +223,7 @@ class NativeNet:
                 self._seen_shapes.popitem(last=False)
             if seen < 2 or self.graph_cache_size == 0:
                 self.last_from_graph = False
-                return self.forward(x)
+                return self.forward(x, want_sem=want_sem)
             while len(self._graphs) >= self.graph_cache_size:
                 self._graphs.popitem(last=False)          # drops the graph, its workspace and static buffers
             with torch.cuda.device(self.device):
@@ -219,13 +232,13 @@ class NativeNet:
                 side = torch.cuda.Stream()
                 side.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(side):
-                    self.forward(xs)                      # warm-up: one-time attribute/workspace set-up happens here
+                    self.forward(xs, want_sem=want_sem)   # warm-up: one-time attribute/workspace set-up happens here
                     side.synchronize()
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g, stream=side):
-                        y, loss, idx = self.forward(xs)
+                        outs = self.forward(xs, want_sem=want_sem)
                 torch.cuda.current_stream().wait_stream(side)
-                ent = {"graph": g, "x": xs, "y": y, "loss": loss, "idx": idx, "ws": self._ws}
+                ent = {"graph": g, "x": xs, "outs": outs, "ws": self._ws}
                 self._ws = None                           # the captured launches own this workspace from now on
                 self._graphs[key] = ent
         else:
@@ -233,7 +246,7 @@ class NativeNet:
         self.last_from_graph = True
         ent["x"].copy_(x, non_blocking=True)
         ent["graph"].replay()
-        return ent["y"], ent["loss"], ent["idx"]
+        return ent["outs"]
 
     def release_graphs(self):
         """Drop every captured graph (and the workspaces they pin)."""
@@ -249,6 +262,7 @@ class NativeNet:
                 "up1": (B, 2 * h, 2 * w, 256), "up2": (B, 4 * h, 4 * w, 128), "z": (B, h, w, self.e_dim),
                 "zq": (B, h, w, self.e_dim), "after_quant": (B, h, w, 256), "dec0": (B, 2 * h, 2 * w, 256),
                 "dec1": (B, 4 * h, 4 * w, 128), "dec2": (B, 8 * h, 8 * w, 64),
+                "vgg": (B, H // 8, W // 8, 512), "semantic": (B, h, w, 512),
                 **{f"z{k}": (B, h * cs // 32, w * cs // 32, e) for k, (cs, _n, e) in enumerate(self.codebooks) if k}}
 
     def decode_indices(self, indices: torch.Tensor) -> torch.Tensor:

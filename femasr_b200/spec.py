@@ -62,14 +62,36 @@ def normalize_codebooks(codebooks, n_e: int = 1024, e_dim: int = 256):
     return cbs
 
 
-def param_spec(scale: int, e_dim: int, n_e: int = 1024, in_channel: int = 3, codebooks=None):
+# VGG19 `features` up to relu4_4 (vgg_arch.py:27-32, 55-139): conv name, Cin, Cout; every conv is 3x3 pad 1
+VGG_CONVS = [("conv1_1", 3, 64), ("conv1_2", 64, 64), ("conv2_1", 64, 128), ("conv2_2", 128, 128),
+             ("conv3_1", 128, 256), ("conv3_2", 256, 256), ("conv3_3", 256, 256), ("conv3_4", 256, 256),
+             ("conv4_1", 256, 512), ("conv4_2", 512, 512), ("conv4_3", 512, 512), ("conv4_4", 512, 512)]
+# index of each conv in torchvision's vgg19().features (the layout of vgg19-dcbb9e9d.pth)
+VGG_TORCHVISION_INDEX = [0, 2, 5, 7, 10, 12, 14, 16, 19, 21, 23, 25]
+VGG_MEAN = (0.485, 0.456, 0.406)       # vgg_arch.py:133-136
+VGG_STD = (0.229, 0.224, 0.225)
+
+
+def semantic_spec() -> List[Tuple[str, tuple, str, int]]:
+    """The 28 tensors use_semantic_loss=True adds (femasr_arch.py:301-309): conv_semantic = Sequential(Conv2d(512, 512, 1),
+    ReLU) and VGGFeatureExtractor(['relu4_4']) with its mean / std buffers."""
+    spec = _conv("conv_semantic.0", 512, 512, 1)
+    spec += [("vgg_feat_extractor.mean", (1, 3, 1, 1), "vgg_mean", 0), ("vgg_feat_extractor.std", (1, 3, 1, 1), "vgg_std", 0)]
+    for name, ci, co in VGG_CONVS:
+        p = f"vgg_feat_extractor.vgg_net.{name}"
+        spec += [(f"{p}.weight", (co, ci, 3, 3), "vgg_w", co * 9), (f"{p}.bias", (co,), "vgg_b", co * 9)]
+    return spec
+
+
+def param_spec(scale: int, e_dim: int, n_e: int = 1024, in_channel: int = 3, codebooks=None, semantic: bool = False):
     """Ordered [(name, shape, kind, fan_in)].  scale 4 | 2: LQ_stage=True;
     scale 1: the HQ autoencoder (LQ_stage=False, femasr_arch.py:241: scale_factor forced to 1; no Swin, no up branches).
     ``codebooks`` = [(scale, n_e, e_dim), ...] for the multi-scale variant (femasr_arch.py:280-299); default: one
-    codebook (32, n_e, e_dim).
+    codebook (32, n_e, e_dim).  ``semantic``: append the use_semantic_loss tensors (semantic_spec()).
 
     kind: w | b (kaiming-uniform bound 1/sqrt(fan_in)), norm_w | norm_b, rpb (trunc-normal .02),
-    rpi | mask (buffers), codebook (U(+-1/n_e)).
+    rpi | mask (buffers), codebook (U(+-1/n_e)), vgg_w | vgg_b (torchvision's VGG init: N(0, 2 / (9 Cout)) | 0;
+    fan_in carries 9 Cout), vgg_mean | vgg_std (the extractor's constant buffers).
     """
     d = encode_depth(scale)
     res = GT_RES // scale
@@ -113,6 +135,8 @@ def param_spec(scale: int, e_dim: int, n_e: int = 1024, in_channel: int = 3, cod
         spec.append((f"quantize_group.{k}.embedding.weight", (ne, ed), "codebook", ne))
         spec += _conv(f"before_quant_group.{k}", ch if k == 0 else 2 * ch, ed, 1)
         spec += _conv(f"after_quant_group.{k}.conv", ed if k == 0 else cbs[k - 1][2] + ed, ch, 3)
+    if semantic:
+        spec += semantic_spec()
     return spec
 
 
@@ -148,17 +172,19 @@ def _gen(seed: int, name: str) -> torch.Generator:
 
 
 def random_state_dict(scale: int, e_dim: int, seed: int = 0, init: str = "default",
-                      n_e: int = 1024, codebooks=None) -> Dict[str, torch.Tensor]:
+                      n_e: int = 1024, codebooks=None, semantic: bool = False) -> Dict[str, torch.Tensor]:
     """Seeded random weights with the reference's default-init distributions.
 
     Each tensor is drawn from its own generator keyed by (seed, name), so the dict is reproducible
     anywhere without the reference.  ``init='default'``: exactly the reference's distributions
     (conv/linear U(+-1/sqrt(fan_in)); GN/LN weight 1 bias 0; rel-pos table trunc-normal(.02),
     network_swinir.py:111; codebook U(+-1/n_e), femasr_arch.py:33).  ``init='perturbed'``: norm affine
-    parameters and the codebook get non-trivial values so tests exercise them.
+    parameters and the codebook get non-trivial values so tests exercise them.  ``semantic``: also the use_semantic_loss
+    tensors; VGG weights N(0, 2 / (9 Cout)) like torchvision's VGG init, VGG biases 0 (default) or small random values
+    (perturbed), conv_semantic kaiming-uniform.
     """
     sd: Dict[str, torch.Tensor] = {}
-    for name, shape, kind, fan_in in param_spec(scale, e_dim, n_e, codebooks=codebooks):
+    for name, shape, kind, fan_in in param_spec(scale, e_dim, n_e, codebooks=codebooks, semantic=semantic):
         g = _gen(seed, name)
         if kind in ("w", "b"):
             bound = 1.0 / math.sqrt(fan_in)
@@ -183,7 +209,23 @@ def random_state_dict(scale: int, e_dim: int, seed: int = 0, init: str = "defaul
                 t = (torch.rand(shape, generator=g) * 2 - 1) / fan_in      # fan_in carries this codebook's n_e
             else:
                 t = torch.randn(shape, generator=g) * 0.5
+        elif kind in ("vgg_w", "vgg_b", "vgg_mean", "vgg_std"):
+            t = vgg_init(shape, kind, fan_in, g, init)
         else:
             raise ValueError(kind)
         sd[name] = t.contiguous()
     return sd
+
+
+def vgg_init(shape, kind: str, fan_out: int, g: torch.Generator = None, init: str = "default") -> torch.Tensor:
+    """VGG extractor tensors: torchvision's VGG init (kaiming-normal fan_out / relu: N(0, 2 / fan_out), bias 0; biases
+    N(0, 0.01^2) for ``init='perturbed'``) and the ImageNet mean / std buffers."""
+    if kind == "vgg_w":
+        return torch.randn(shape, generator=g) * math.sqrt(2.0 / fan_out)
+    if kind == "vgg_b":
+        return torch.randn(shape, generator=g) * 0.01 if init == "perturbed" else torch.zeros(shape)
+    if kind == "vgg_mean":
+        return torch.tensor(VGG_MEAN).view(shape)
+    if kind == "vgg_std":
+        return torch.tensor(VGG_STD).view(shape)
+    raise ValueError(kind)

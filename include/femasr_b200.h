@@ -73,6 +73,21 @@ int femasr_net_params_complete(femasr_net* net);
 /* Bytes of device workspace femasr_net_forward needs for a [B,3,H,W] input. */
 int femasr_net_workspace_bytes(femasr_net* net, int B, int H, int W, size_t* bytes);
 
+/* HQ-stage semantic loss (use_semantic_loss=True, femasr_arch.py:301-309, 318-320, 344-347, 372).  Call after
+ * femasr_net_create and before any set_param: adds the 28 tensors conv_semantic.0.{weight,bias},
+ * vgg_feat_extractor.{mean,std} (3 floats each) and vgg_feat_extractor.vgg_net.convX_Y.{weight,bias} (VGG19 up to
+ * relu4_4) to the net's parameters; femasr_net_params_complete then requires them. */
+int femasr_net_enable_semantic(femasr_net* net);
+/* Workspace of femasr_net_forward_sem; with_sem = 0 is femasr_net_workspace_bytes. */
+int femasr_net_workspace_bytes_sem(femasr_net* net, int B, int H, int W, int with_sem, size_t* bytes);
+/* femasr_net_forward_gt plus sem_loss (1 float device) = sum over quantising levels of
+ * mse(ReLU(conv_semantic(z_quant)), VGG19 relu4_4((x - mean) / std)).  It exists only where the shapes agree: the HQ
+ * stage (scale_factor 1), one codebook at 32 with e_dim 512; anything else returns FEMASR_ERR_ARG naming both shapes
+ * (the reference raises from conv_semantic / mse_loss).  sem_loss == NULL is exactly femasr_net_forward_gt. */
+int femasr_net_forward_sem(femasr_net* net, const float* x_nchw, float* y_nchw, int64_t* indices,
+                           float* cb_loss, const int64_t* gt_indices, float* sem_loss, int B, int H, int W,
+                           void* workspace, size_t workspace_bytes, void* stream);
+
 /* encode_and_decode (femasr_arch.py:311-374).
  *   x_nchw    [B,3,H,W] fp32 device.  H,W such that the Swin stage (H/2 for x4, H/4 for x2) is a
  *             multiple of 8, else FEMASR_ERR_ARG (the reference raises from window_partition).
@@ -101,7 +116,8 @@ int femasr_net_decode_workspace_bytes(femasr_net* net, int B, int h, int w, size
 /* Stage taps for parity tests: when `dst` is set for a stage name, the next forward copies that
  * stage's NHWC fp32 tensor there (device, `capacity` floats).  Names: in_conv, down, swin, up1, up2,
  * z, zq, after_quant, dec0, dec1, dec2 (z / zq / after_quant: first codebook), z1, z2 (features in front of the
- * second / third codebook).  dst == NULL removes the tap. */
+ * second / third codebook), vgg (relu4_4) and semantic (ReLU(conv_semantic(z_quant))), the last two only in a
+ * forward that computes the semantic loss.  dst == NULL removes the tap. */
 int femasr_net_set_tap(femasr_net* net, const char* stage, float* dst, size_t capacity);
 /* Number of kernels the last femasr_net_forward launched (bench.py's gpu_launches). */
 int femasr_net_last_launch_count(femasr_net* net);
@@ -140,8 +156,11 @@ int femasr_pack_weight(const float* w_oihw, float* w_packed, int Cout, int Cin, 
 enum { FEMASR_PRO_NONE = 0, FEMASR_PRO_GN_SILU = 1, FEMASR_PRO_LN = 2,
        /* femasr_tc_prepare only: GN + SiLU with ex2.approx / rcp.approx (relative error <= 4e-7 instead of 1.2e-7);
           the engine uses it behind the VQ, where the bar is 1e-3 on the output, never in front of the index decision */
-       FEMASR_PRO_GN_SILU_FAST = 3 };
-enum { FEMASR_ACT_NONE = 0, FEMASR_ACT_GELU = 1 };
+       FEMASR_PRO_GN_SILU_FAST = 3,
+       /* femasr_tc_prepare only: 2x2 stride-2 max-pool (nn.MaxPool2d(2, 2), floor) of the fp32 input before the split;
+          H, W are the INPUT dims and a_hi/a_lo are [B,H/2,W/2,C] */
+       FEMASR_PRO_MAXPOOL2 = 4 };
+enum { FEMASR_ACT_NONE = 0, FEMASR_ACT_GELU = 1, FEMASR_ACT_RELU = 2 /* bias first, then max(v, 0) */ };
 
 /* Implicit-GEMM convolution / linear:  y = act(conv(pro(x)) + bias) + res1 + res2.
  *   ksize 3 (pad 1) or 1 (pad 0); stride 1|2; upsample=1 applies nearest x2 to pro(x) first
@@ -314,6 +333,19 @@ int femasr_in_conv4x4_split(const float* x_nchw, const float* w, const float* bi
  * femasr_tc_igemm with ksize 1, Cin 64 on a weight blob packed from femasr_in_conv_pad_weight's [Cout][64] matrix. */
 int femasr_in_conv_im2col(const float* x_nchw, void* a_hi, void* a_lo, int B, int Cin, int H, int W, void* stream);
 int femasr_in_conv_pad_weight(const float* w_oihw, float* w_padded, int Cout, void* stream);
+/* VGG19 conv1_1 (vgg_arch.py:55-139) as the same kind of GEMM: femasr_vgg_im2col normalises the image,
+ * (x - mean[c]) / std[c] with a true fp32 division, and writes per pixel the 27 values of the 3x3 pad-1 window
+ * (k = (kh*3+kw)*3+ci, zero padded to 64; the padding is zero AFTER normalisation like F.conv2d's) either as split fp16
+ * planes a_hi/a_lo [B*H*W][64] (a_f32 NULL) or as fp32 rows a_f32 [B*H*W][64] (a_hi/a_lo NULL).
+ * femasr_vgg_pad_weight: OIHW [Cout,3,3,3] -> [Cout][64] in that K order. */
+int femasr_vgg_im2col(const float* x_nchw, const float* mean, const float* std_, void* a_hi, void* a_lo, float* a_f32,
+                      int B, int H, int W, void* stream);
+int femasr_vgg_pad_weight(const float* w_oihw, float* w_padded, int Cout, void* stream);
+/* nn.MaxPool2d(2, 2) on fp32 NHWC: x [B,H,W,C] -> y [B,H/2,W/2,C] (the gemm_path 0 form of FEMASR_PRO_MAXPOOL2). */
+int femasr_maxpool2(const float* x, float* y, int B, int H, int W, int C, void* stream);
+/* rows[i] = sum_c (a[i][c] - b[i][c])^2 over [N, C] fp32, in a fixed order (one warp per row); the mean is then
+ * femasr_sum_scaled(rows, out, N, 1 / (N * C)). */
+int femasr_sq_diff_rows(const float* a, const float* b, float* rows, int N, int C, void* stream);
 /* out_conv (femasr_arch.py:273): 3x3 pad 1, NHWC [B,H,W,Cin] -> NCHW [B,3,H,W].  w packed [9*Cin][3]. */
 int femasr_out_conv3x3(const float* x_nhwc, const float* w, const float* bias, float* y_nchw, int B,
                        int H, int W, int Cin, void* stream);
