@@ -70,15 +70,34 @@ struct Arena {
   }
 };
 
-struct DevBuf {
-  float* p = nullptr;
-  size_t n = 0;
-};
+
+// The device forms femasr_net_set_param packs a parameter into, besides its fp32 copy in the reference layout.  The spec
+// decides them once from the layer's role and the net's configuration; the graph reads the same flags.
+constexpr unsigned
+  FORM_KMAJOR = 1u << 0,   // K-major fp32 GEMM operand (conv / linear weight; codebook^T): the SIMT GEMM's weight
+  FORM_TC = 1u << 1,       // split-fp16 blob: the tensor-core GEMM's weight (codebook: the fused VQ's B operand)
+  FORM_TC8 = 1u << 2,      // the same in the F8 cross-term packing (3x3 convs that may run behind the VQ)
+  FORM_UP = 1u << 3,       // sub-pixel phase filters of a nearest-x2 -> conv3x3 site, split fp16
+  FORM_UP8 = 1u << 4,      // the same in the F8 packing
+  FORM_IM2COL = 1u << 5,   // [Cout][64] zero-padded im2col matrix (in_conv, VGG conv1_1): split-fp16 blob on gemm_path 1,
+                           // K-major fp32 on gemm_path 0
+  FORM_RELB = 1u << 6,     // rel-pos table expanded to [8][64][64] (SIMT attention) and in the mma kernel's fragment order
+  FORM_ESQ = 1u << 7;      // sum e^2 per codebook row
 
 struct ParamInfo {
   size_t numel;
-  int kind;  // 0 plain, 1 conv/linear weight [Cout,Cin,k,k], 2 rel-pos table, 3 codebook
-  int Cout, Cin, k;
+  int Cout, Cin, k;   // conv / linear weight [Cout,Cin,k,k]; codebook [n_e,e_dim] as Cout, Cin, k = 1
+  unsigned forms;     // FORM_*
+};
+
+// every device buffer of one parameter; nullptr where its ParamInfo lists no such form
+struct DevParam {
+  float* raw = nullptr;        // fp32 copy in the reference layout
+  float* packed = nullptr;     // FORM_KMAJOR, or the expanded rel bias of FORM_RELB
+  float* relb_mma = nullptr;   // FORM_RELB, fragment order
+  float* esq = nullptr;        // FORM_ESQ
+  void *tc = nullptr, *tc8 = nullptr, *up = nullptr, *up8 = nullptr, *im2col = nullptr;
+  void release() { for (void* p : {(void*)raw, (void*)packed, (void*)relb_mma, (void*)esq, tc, tc8, up, up8, im2col}) cudaFree(p); }
 };
 
 struct Tap { float* dst; size_t cap; };
@@ -94,13 +113,7 @@ struct femasr_net {
   int depth;   // encode depth (1 for x4, 2 for x2, 3 for the HQ autoencoder)
   bool hq = false;   // scale_factor 1: LQ_stage=False graph (no Swin, no up branches, no skip adds)
   std::map<std::string, ParamInfo> spec;
-  std::map<std::string, DevBuf> raw;      // fp32 copy in the reference layout
-  std::map<std::string, DevBuf> packed;   // K-major GEMM operand / expanded rel bias / codebook^T
-  std::map<std::string, DevBuf> packed_mma;   // rel-pos bias in the mma attention kernel's fragment order
-  std::map<std::string, DevBuf> tcw;      // tensor-core operand (split fp16), gemm_path 1
-  std::map<std::string, DevBuf> tcw_up;   // sub-pixel phase filters of the upsample-fused 3x3 convs
-  std::map<std::string, DevBuf> tcw8, tcw_up8;   // the same two in the F8 cross-term packing (layers behind the VQ)
-  std::map<std::string, DevBuf> esq;      // sum e^2 per codebook row, keyed by the codebook's parameter name
+  std::map<std::string, DevParam> dev;
   struct Codebook { int scale, n_e, e_dim; };
   std::vector<Codebook> cbs;              // codebook_params rows; cbs[0].scale == 32
   int level_cb[3] = {0, -1, -1};          // decoder level i (resolution 32 << i) -> codebook index or -1
@@ -109,9 +122,7 @@ struct femasr_net {
   int last_launches = 0;
   bool profile = false;
   bool tc_precise = true;                 // K-sliced fp32 accumulation for the layers in front of the VQ
-  bool oc_mma = true;                     // out_conv on mma.sync in the tensor-core path (FEMASR_OUTCONV_MMA=0: SIMT kernel)
   bool f8_cross = true;                   // layers behind the VQ: the two cross products of the split as one fp8 product (FEMASR_F8_CROSS=0: three fp16 products)
-  bool in_conv_tc = true;                 // in_conv as an im2col GEMM on the tensor cores (FEMASR_IN_CONV_TC=0: fp32 SIMT kernel)
   int tc_slice_kb = 4;                    // K-slice length in 64-wide k-blocks (FEMASR_TC_SLICE_KB; study knob)
   bool vq_fused = true;                   // VQ distances on the tensor cores with the argmin fused (FEMASR_VQ_FUSED=0: fp32 SIMT z.E^T + vq_select)
   bool fast_silu = true;                  // approximate-unit SiLU in the operand staging behind the VQ (FEMASR_FAST_SILU=0: exact)
@@ -121,14 +132,7 @@ struct femasr_net {
   std::string prof_json;
   ~femasr_net() {
     for (auto& r : prof) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
-    for (auto& kv : raw) cudaFree(kv.second.p);
-    for (auto& kv : packed) cudaFree(kv.second.p);
-    for (auto& kv : packed_mma) cudaFree(kv.second.p);
-    for (auto& kv : tcw) cudaFree(kv.second.p);
-    for (auto& kv : tcw_up) cudaFree(kv.second.p);
-    for (auto& kv : tcw8) cudaFree(kv.second.p);
-    for (auto& kv : tcw_up8) cudaFree(kv.second.p);
-    for (auto& kv : esq) cudaFree(kv.second.p);
+    for (auto& kv : dev) kv.second.release();
   }
 };
 
@@ -139,8 +143,19 @@ static int chan(int res) {
   return -1;
 }
 
-static void add_conv(femasr_net* n, const std::string& p, int ci, int co, int k) {
-  n->spec[p + ".weight"] = ParamInfo{(size_t)co * ci * k * k, 1, co, ci, k};
+enum Role { CONV, UP_CONV, IN_CONV, VGG_CONV, VGG_CONV1 };
+
+static unsigned weight_forms(const femasr_net* n, Role r, int ci, int co, int k) {
+  const bool tc = n->cfg.gemm_path == 1;
+  if (r == VGG_CONV1 || (r == IN_CONV && tc)) return FORM_KMAJOR | FORM_IM2COL;   // K = 27 / 48 zero-padded to 64
+  if (!tc || (k != 1 && k != 3) || ci % 64 || co % 64) return FORM_KMAJOR;
+  unsigned f = FORM_KMAJOR | FORM_TC;
+  if (n->f8_cross && k == 3 && r != VGG_CONV) f |= FORM_TC8;      // may run behind the VQ; the VGG convs never use F8
+  if (r == UP_CONV) f |= FORM_UP | (n->f8_cross ? FORM_UP8 : 0);
+  return f;
+}
+static void add_conv(femasr_net* n, const std::string& p, int ci, int co, int k, Role r = CONV) {
+  n->spec[p + ".weight"] = ParamInfo{(size_t)co * ci * k * k, co, ci, k, weight_forms(n, r, ci, co, k)};
   n->spec[p + ".bias"] = ParamInfo{(size_t)co, 0, 0, 0, 0};
 }
 static void add_vec(femasr_net* n, const std::string& name, size_t c) { n->spec[name] = ParamInfo{c, 0, 0, 0, 0}; }
@@ -150,13 +165,19 @@ static void add_resblock(femasr_net* n, const std::string& p, int c) {
   add_vec(n, p + ".conv.3.norm.weight", c); add_vec(n, p + ".conv.3.norm.bias", c);
   add_conv(n, p + ".conv.5", c, c, 3);
 }
+// nearest-x2 -> conv3x3 (p.1) -> ResBlock (p.2) -> ResBlock (p.3): femasr_arch.py:168-180, 195-211
+static void add_up_block(femasr_net* n, const std::string& p, int ci, int co) {
+  add_conv(n, p + ".1", ci, co, 3, UP_CONV);
+  add_resblock(n, p + ".2", co);
+  add_resblock(n, p + ".3", co);
+}
 
 static void build_spec(femasr_net* n) {
   const int scale = n->cfg.scale_factor;
   const int d = n->depth;
   int res = 256 / scale;
   const std::string enc = "multiscale_encoder";
-  add_conv(n, enc + ".in_conv", n->cfg.in_channel, chan(res), 4);
+  add_conv(n, enc + ".in_conv", n->cfg.in_channel, chan(res), 4, IN_CONV);
   for (int i = 0; i < d; ++i) {
     const std::string b = enc + ".blocks." + std::to_string(i);
     add_conv(n, b + ".0", chan(res), chan(res / 2), 3);
@@ -169,7 +190,7 @@ static void build_spec(femasr_net* n) {
     for (int b = 0; b < 6; ++b) {
       const std::string p = sw + std::to_string(r) + ".residual_group.blocks." + std::to_string(b);
       add_vec(n, p + ".norm1.weight", 256); add_vec(n, p + ".norm1.bias", 256);
-      n->spec[p + ".attn.relative_position_bias_table"] = ParamInfo{225 * 8, 2, 0, 0, 0};
+      n->spec[p + ".attn.relative_position_bias_table"] = ParamInfo{225 * 8, 0, 0, 0, FORM_RELB};
       add_conv(n, p + ".attn.qkv", 256, 768, 1);
       add_conv(n, p + ".attn.proj", 256, 256, 1);
       add_vec(n, p + ".norm2.weight", 256); add_vec(n, p + ".norm2.bias", 256);
@@ -179,25 +200,17 @@ static void build_spec(femasr_net* n) {
     add_conv(n, sw + std::to_string(r) + ".conv", 256, 256, 3);
   }
   for (int j = d + 1; j <= (n->hq ? d : d + 2); ++j) {
-    const std::string b = enc + ".blocks." + std::to_string(j);
-    add_conv(n, b + ".1", chan(res), chan(res * 2), 3);
-    add_resblock(n, b + ".2", chan(res * 2));
-    add_resblock(n, b + ".3", chan(res * 2));
+    add_up_block(n, enc + ".blocks." + std::to_string(j), chan(res), chan(res * 2));
     res *= 2;
   }
-  for (int i = 0; i < 3; ++i) {
-    const int r = 32 << i;
-    const std::string b = "decoder_group." + std::to_string(i) + ".block";
-    add_conv(n, b + ".1", chan(r), chan(r * 2), 3);
-    add_resblock(n, b + ".2", chan(r * 2));
-    add_resblock(n, b + ".3", chan(r * 2));
-  }
+  for (int i = 0; i < 3; ++i) add_up_block(n, "decoder_group." + std::to_string(i) + ".block", chan(32 << i), chan(64 << i));
   add_conv(n, "out_conv", 64, 3, 3);
+  const unsigned cb_forms = FORM_KMAJOR | FORM_ESQ | (n->cfg.gemm_path == 1 && n->vq_fused ? FORM_TC : 0);
   for (size_t k = 0; k < n->cbs.size(); ++k) {           // femasr_arch.py:280-299
     const femasr_net::Codebook& cb = n->cbs[k];
     const std::string ks = std::to_string(k);
     const int ch = chan(cb.scale);
-    n->spec["quantize_group." + ks + ".embedding.weight"] = ParamInfo{(size_t)cb.n_e * cb.e_dim, 3, cb.n_e, cb.e_dim, 1};
+    n->spec["quantize_group." + ks + ".embedding.weight"] = ParamInfo{(size_t)cb.n_e * cb.e_dim, cb.n_e, cb.e_dim, 1, cb_forms};
     add_conv(n, "before_quant_group." + ks, k == 0 ? ch : 2 * ch, cb.e_dim, 1);
     add_conv(n, "after_quant_group." + ks + ".conv", k == 0 ? cb.e_dim : n->cbs[k - 1].e_dim + cb.e_dim, ch, 3);
   }
@@ -212,36 +225,91 @@ static const bool VGG_POOL_BEFORE[12] = {false, false, true, false, true, false,
 
 // use_semantic_loss=True (femasr_arch.py:301-309): conv_semantic = Sequential(Conv2d(512, 512, 1), ReLU) and the extractor
 static void add_semantic(femasr_net* n) {
-  add_conv(n, "conv_semantic.0", 512, 512, 1);
+  add_conv(n, "conv_semantic.0", 512, 512, 1, VGG_CONV);
   add_vec(n, "vgg_feat_extractor.mean", 3);
   add_vec(n, "vgg_feat_extractor.std", 3);
   int cin = 3;
   for (int i = 0; i < 12; ++i) {
-    add_conv(n, std::string("vgg_feat_extractor.vgg_net.") + VGG_CONVS[i], cin, VGG_COUT[i], 3);
+    add_conv(n, std::string("vgg_feat_extractor.vgg_net.") + VGG_CONVS[i], cin, VGG_COUT[i], 3, i == 0 ? VGG_CONV1 : VGG_CONV);
     cin = VGG_COUT[i];
   }
 }
 
 // ---------------------------------------------------------------------------------------------
+// One conv / linear layer of the graph.  H, W: the conv-input size (low-res when upsample).  The operand is fp32 x, or
+// split-fp16 planes a_hi/a_lo a producer already wrote (tensor-core GEMM only); the result is fp32 y, or split planes
+// o_hi/o_lo for the next tensor-core GEMM.
+struct ConvDesc {
+  std::string w;                                   // parameter prefix: w.weight, w.bias
+  const char* name = nullptr;                      // profile name (nullptr: "igemm_simt" / "tc_igemm" with detail labels)
+  const float* x = nullptr;
+  const void *a_hi = nullptr, *a_lo = nullptr;
+  float* y = nullptr;
+  void *o_hi = nullptr, *o_lo = nullptr;
+  int B = 0, H = 0, W = 0, Cin = 0, Cout = 0, k = 3;
+  int stride = 1, upsample = 0;
+  int pro = FEMASR_PRO_NONE;                       // prologue; pa/pb: GN scale/shift or LN mean/rstd tables
+  const float *pa = nullptr, *pb = nullptr, *gamma = nullptr, *beta = nullptr;
+  int act = FEMASR_ACT_NONE;
+  const float *res1 = nullptr, *res2 = nullptr;
+  float* gn_partial = nullptr;                     // GroupNorm partials of the output (tensor-core GEMM)
+  bool bias = true;
+  bool im2col = false;                             // the weight's FORM_IM2COL: a 1x1 GEMM over 64-wide im2col rows
+  bool semantic = false;                           // a GEMM of the semantic branch (its own numerics)
+  int macs = 0;                                    // algorithmic MACs per output element if not Cin*k*k (im2col GEMMs)
+};
+
+static ConvDesc geom(const std::string& w, int B, int H, int W, int Cin, int Cout, int k) {
+  ConvDesc d;
+  d.w = w; d.B = B; d.H = H; d.W = W; d.Cin = Cin; d.Cout = Cout; d.k = k;
+  return d;
+}
+
+static double conv_flops(const ConvDesc& d) {   // algorithmic (reference) count
+  const int u = d.upsample ? 2 : 1;
+  const int Ho = d.stride == 2 ? (d.H - 1) / 2 + 1 : d.H * u, Wo = d.stride == 2 ? (d.W - 1) / 2 + 1 : d.W * u;
+  return 2.0 * d.B * Ho * (double)Wo * d.Cout * (d.macs ? d.macs : d.Cin * d.k * d.k);
+}
+
+// How a tensor-core conv computes: K-slicing, the F8 cross product and the staging prologue
+struct Numerics { int slice_kb = 0; bool f8 = false; int prologue = FEMASR_PRO_NONE; };
+
 struct Ctx {
   femasr_net* net;
   Arena ar;
   cudaStream_t st;
+  long l0;                       // g_launches when the run started
   int status = FEMASR_OK;
+  double flops = 0;              // sizing run: sum of the launches' algorithmic FLOPs
   float* sem_loss = nullptr;     // forward_sem: the semantic loss output (non-NULL = run the VGG branch)
   float* vgg_feat = nullptr;     // relu4_4 [B,H/8,W/8,512], alive from the VGG stage to the loss at quantising level 0
   bool precise_region = false;   // true while emitting the layers in front of the VQ (index-critical)
+
+  // workspace == nullptr: a sizing run (allocations and FLOPs only, nothing launched); else a run over the caller's
+  // workspace, aligned up to 256 bytes
+  Ctx(femasr_net* n, void* workspace, size_t bytes, void* stream) : net(n), st(as_stream(stream)), l0(g_launches) {
+    const uintptr_t mis = (256 - ((uintptr_t)workspace & 255)) & 255;
+    ar.dry = !workspace;
+    ar.base = ar.dry ? reinterpret_cast<char*>(uintptr_t(1) << 40) : reinterpret_cast<char*>(workspace) + mis;
+    ar.cap = ar.dry ? 0 : bytes - mis;
+  }
   bool dry() const { return ar.dry; }
   bool ok() const { return status == FEMASR_OK; }
   void check(int s) { if (status == FEMASR_OK && s != FEMASR_OK) status = s; }
+  size_t bytes_needed() const { return ar.peak + 256; }
+  int finish() {
+    if (!dry()) net->last_launches = (int)(g_launches - l0);
+    return status;
+  }
 
   // every kernel launch of the graph goes through here; in profile mode it is bracketed by CUDA events
   template <class F>
-  void run(const char* name, double flops, F&& f) {
-    if (dry() || !ok()) return;
+  void run(const char* name, double fl, F&& f) {
+    if (dry()) { flops += fl; return; }
+    if (!ok()) return;
     if (ar.overflow) { check(fail(FEMASR_ERR_STATE, "workspace plan mismatch: the graph needs more than femasr_net_workspace_bytes reported")); return; }
     if (net->profile) {
-      ProfRec r{name, flops, nullptr, nullptr};
+      ProfRec r{name, fl, nullptr, nullptr};
       cudaEventCreate(&r.e0); cudaEventCreate(&r.e1);
       cudaEventRecord(r.e0, st);
       check(f());
@@ -263,147 +331,126 @@ struct Ctx {
     return names.insert(s).first->c_str();
   }
 
-  const float* P(const std::string& name) {      // packed (or raw when there is no packed form)
-    if (dry()) return nullptr;
-    auto it = net->packed.find(name);
-    if (it != net->packed.end()) return it->second.p;
-    auto jt = net->raw.find(name);
-    if (jt == net->raw.end()) { check(fail(FEMASR_ERR_STATE, "parameter not set: " + name)); return nullptr; }
-    return jt->second.p;
+  // a parameter's device buffers: all nullptr in a sizing run, and for a parameter that was never set (which fails the run)
+  const DevParam& D(const std::string& name) {
+    static const DevParam none;
+    if (dry()) return none;
+    auto it = net->dev.find(name);
+    if (it == net->dev.end()) { check(fail(FEMASR_ERR_STATE, "parameter not set: " + name)); return none; }
+    return it->second;
   }
-  const void* TCW(const std::string& name) {
-    auto it = net->tcw.find(name);
-    return it == net->tcw.end() ? nullptr : it->second.p;
+  const float* P(const std::string& name) {      // packed (or raw when there is no packed form)
+    const DevParam& d = D(name);
+    return d.packed ? d.packed : d.raw;
+  }
+  bool has(const std::string& name, unsigned form) const { return (net->spec.at(name).forms & form) != 0; }
+  bool tapped(const char* stage) const {
+    auto it = net->taps.find(stage);
+    return it != net->taps.end() && it->second.dst;
   }
   void tap(const char* stage, const float* src, size_t n) {
-    if (dry() || !ok()) return;
-    auto it = net->taps.find(stage);
-    if (it == net->taps.end() || !it->second.dst) return;
-    if (it->second.cap < n) { check(fail(FEMASR_ERR_ARG, std::string("tap buffer too small: ") + stage)); return; }
-    cudaError_t e = cudaMemcpyAsync(it->second.dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
+    if (dry() || !ok() || !tapped(stage)) return;
+    const Tap& t = net->taps.at(stage);
+    if (t.cap < n) { check(fail(FEMASR_ERR_ARG, std::string("tap buffer too small: ") + stage)); return; }
+    cudaError_t e = cudaMemcpyAsync(t.dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
     if (e != cudaSuccess) check(fail(FEMASR_ERR_CUDA, cudaGetErrorString(e)));
   }
 
-  // y = conv(x) (+epilogue); wname is the conv's parameter prefix.
-  void conv(const std::string& wname, const float* x, float* y, int B, int Hin, int Win, int Cin, int Cout, int ksize,
-            int stride, int upsample, int prologue, const float* pa, const float* pb, const float* gamma,
-            const float* beta, int act, const float* res1, const float* res2, bool has_bias = true) {
-    if (has_bias && tc_eligible(wname, Cin, Cout, ksize, stride, upsample)) {
-      conv_tc(wname, x, y, B, Hin, Win, Cin, Cout, ksize, upsample, prologue, pa, pb, gamma, beta, act, res1, res2,
-              nullptr, nullptr, nullptr, nullptr, nullptr, stride);
+  // the wgmma implicit GEMM wherever the spec gave the weight its tensor-core form (gemm_path 1), else the SIMT one
+  bool use_tc(const ConvDesc& d) const {
+    return net->cfg.gemm_path == 1 && (d.im2col || has(d.w + ".weight", d.upsample ? FORM_UP : FORM_TC));
+  }
+
+  // The numerics policy.  In front of the VQ (index-critical): every tc_slice_kb k-blocks the tensor core's truncating
+  // accumulator is folded into an fp32 round-to-nearest running sum (see femasr_tc_args.slice_kb).  Behind it (bar: 1e-3
+  // on the output): approximate-unit SiLU, and the two cross products of the split as one fp8 product.  The semantic
+  // branch runs in one pass (or FEMASR_SEM_SLICE_KB) without F8, wherever in the graph it sits.
+  Numerics numerics(const ConvDesc& d) const {
+    Numerics m;
+    m.prologue = d.pro;
+    if (d.semantic) {
+      m.slice_kb = net->sem_slice_kb;
+    } else if (precise_region) {
+      const int nkb = (d.upsample ? 4 : d.k * d.k) * (d.Cin / 64);
+      if (net->tc_precise && nkb > net->tc_slice_kb) m.slice_kb = net->tc_slice_kb;
+    } else {
+      m.f8 = !d.a_hi && d.k == 3 && d.pro != FEMASR_PRO_LN && has(d.w + ".weight", d.upsample ? FORM_UP8 : FORM_TC8);
+      if (d.pro == FEMASR_PRO_GN_SILU && net->fast_silu) m.prologue = FEMASR_PRO_GN_SILU_FAST;
+    }
+    return m;
+  }
+
+  const void* weight(const ConvDesc& d, bool tc, bool f8) {
+    const DevParam& p = D(d.w + ".weight");
+    const void* w = d.im2col ? p.im2col : !tc ? p.packed : d.upsample ? (f8 ? p.up8 : p.up) : (f8 ? p.tc8 : p.tc);
+    if (!dry() && !w) check(fail(FEMASR_ERR_STATE, "parameter not packed: " + d.w + ".weight"));
+    return w;
+  }
+
+  // the tensor-core GEMM's arguments for d over the operand planes a_hi/a_lo
+  femasr_tc_args tc_args(const ConvDesc& d, const Numerics& m, const void* a_hi, const void* a_lo) {
+    femasr_tc_args t;
+    memset(&t, 0, sizeof(t));
+    t.a_hi = a_hi; t.a_lo = a_lo; t.w_blob = weight(d, true, m.f8); t.bias = d.bias ? P(d.w + ".bias") : nullptr;
+    t.res1 = d.res1; t.res2 = d.res2; t.y = d.y; t.out_hi = d.o_hi; t.out_lo = d.o_lo; t.gn_partial = d.gn_partial;
+    t.B = d.B; t.H = d.H; t.W = d.W; t.Cin = d.Cin; t.Cout = d.Cout; t.ksize = d.k; t.act = d.act; t.upsample = d.upsample;
+    t.stride = d.stride; t.slice_kb = m.slice_kb; t.f8 = m.f8 ? 1 : 0; t.pair = -1; t.strip = -1;
+    return t;
+  }
+
+  // y = conv(x) (+epilogue).  The tensor-core path stages the activation operand (prologue + fp16 split, or the F8
+  // plane) unless the producer already wrote split planes; a fused nearest-x2 upsample runs as four sub-pixel 2x2 convs
+  // on the low-res operand.  Allocation happens in sizing runs too.
+  void conv(const ConvDesc& d) {
+    if (!use_tc(d)) {
+      femasr_igemm_args a;
+      memset(&a, 0, sizeof(a));
+      a.x = d.x; a.w = static_cast<const float*>(weight(d, false, false)); a.bias = d.bias ? P(d.w + ".bias") : nullptr;
+      a.res1 = d.res1; a.res2 = d.res2; a.y = d.y; a.pro_a = d.pa; a.pro_b = d.pb; a.gamma = d.gamma; a.beta = d.beta;
+      a.B = d.B; a.Hin = d.H; a.Win = d.W; a.Cin = d.Cin; a.Cout = d.Cout; a.ksize = d.k; a.stride = d.stride;
+      a.upsample = d.upsample; a.prologue = d.pro; a.act = d.act;
+      run(d.name ? d.name : "igemm_simt", conv_flops(d), [&] { return femasr_igemm_simt(&a, st); });
       return;
     }
-    if (dry() || !ok()) return;
-    femasr_igemm_args a;
-    memset(&a, 0, sizeof(a));
-    a.x = x; a.w = P(wname + ".weight"); a.bias = has_bias ? P(wname + ".bias") : nullptr;
-    a.res1 = res1; a.res2 = res2; a.y = y; a.pro_a = pa; a.pro_b = pb; a.gamma = gamma; a.beta = beta;
-    a.B = B; a.Hin = Hin; a.Win = Win; a.Cin = Cin; a.Cout = Cout; a.ksize = ksize; a.stride = stride;
-    a.upsample = upsample; a.prologue = prologue; a.act = act;
-    if (!ok()) return;
-    int Ho, Wo;
-    if (ksize == 1) { Ho = Hin; Wo = Win; }
-    else { const int He = upsample ? 2 * Hin : Hin, We = upsample ? 2 * Win : Win;
-           Ho = stride == 1 ? He : (He - 1) / 2 + 1; Wo = stride == 1 ? We : (We - 1) / 2 + 1; }
-    const double flops = 2.0 * B * Ho * Wo * (double)Cout * Cin * ksize * ksize;
-    run("igemm_simt", flops, [&] { return femasr_igemm_simt(&a, st); });
-  }
-
-  bool tc_eligible(const std::string& wname, int Cin, int Cout, int ksize, int stride, int upsample) const {
-    if (net->cfg.gemm_path != 1 || (ksize != 1 && ksize != 3) || Cin % 64 || Cout % 64) return false;
-    if (stride != 1 && !(stride == 2 && ksize == 3 && !upsample)) return false;
-    if (dry()) return true;
-    return upsample ? net->tcw_up.count(wname + ".weight") != 0 : net->tcw.count(wname + ".weight") != 0;
-  }
-
-  // tensor-core variant of conv(): stage the activation operand (prologue + fp16 split) unless the producer
-  // already wrote split planes (pre_hi/pre_lo), then the wgmma implicit GEMM; optionally the result is
-  // emitted as split planes for the next GEMM (out_hi/out_lo) instead of fp32 y.  A fused nearest-x2 upsample
-  // runs as four sub-pixel 2x2 convs on the low-res operand.  Allocation happens in dry runs too.
-  void conv_tc(const std::string& wname, const float* x, float* y, int B, int Hin, int Win, int Cin, int Cout, int ksize,
-               int upsample, int prologue, const float* pa, const float* pb, const float* gamma, const float* beta,
-               int act, const float* res1, const float* res2, const void* pre_hi = nullptr, const void* pre_lo = nullptr,
-               void* out_hi = nullptr, void* out_lo = nullptr, float* gn_partial = nullptr, int stride = 1,
-               bool precise = false) {
-    const size_t plane_halves = (size_t)B * Hin * Win * Cin;
+    const Numerics m = numerics(d);
     float *ahi = nullptr, *alo = nullptr;
-    if (!pre_hi) {
+    if (!d.a_hi) {
+      const size_t plane_halves = (size_t)d.B * d.H * d.W * d.Cin;
       ahi = ar.alloc((plane_halves + 1) / 2);
       alo = ar.alloc((plane_halves + 1) / 2);
+      run(detail_name(m.f8 ? "tc_prepare_f8" : "tc_prepare", m.prologue, d.Cin, d.Cin, d.H, d.W, 0, 1, 0), 0.0, [&] {
+        return m.f8 ? femasr_tc_prepare_f8(d.x, ahi, alo, m.prologue, d.pa, d.pb, d.B, d.H, d.W, d.Cin, st)
+                    : femasr_tc_prepare(d.x, ahi, alo, m.prologue, d.pa, d.pb, d.gamma, d.beta, d.B, d.H, d.W, d.Cin, 0,
+                                        d.pro == FEMASR_PRO_LN ? 1e-5f : 1e-6f, st);
+      });
     }
-    if (!dry() && ok()) {
-      // behind the VQ (bar: 1e-3 on the output): approximate-unit SiLU, and the two cross products of the split as one
-      // fp8 product (F8 mode: staging writes the interleaved e4m3 plane, the weights come from the F8 packing)
-      const bool relaxed = !precise && !precise_region;
-      const bool f8 = relaxed && net->f8_cross && !pre_hi && ksize == 3 && prologue != FEMASR_PRO_LN &&
-                      (upsample ? net->tcw_up8.count(wname + ".weight") : net->tcw8.count(wname + ".weight")) != 0;
-      if (!pre_hi) {
-        const int pmode = (prologue == FEMASR_PRO_GN_SILU && relaxed && net->fast_silu) ? FEMASR_PRO_GN_SILU_FAST : prologue;
-        run(detail_name(f8 ? "tc_prepare_f8" : "tc_prepare", pmode, Cin, Cin, Hin, Win, 0, 1, 0), 0.0, [&] {
-          return f8 ? femasr_tc_prepare_f8(x, ahi, alo, pmode, pa, pb, B, Hin, Win, Cin, st)
-                    : femasr_tc_prepare(x, ahi, alo, pmode, pa, pb, gamma, beta, B, Hin, Win, Cin, 0,
-                                        prologue == FEMASR_PRO_LN ? 1e-5f : 1e-6f, st);
-        });
-      }
-      femasr_tc_args t;
-      memset(&t, 0, sizeof(t));
-      t.a_hi = pre_hi ? pre_hi : ahi; t.a_lo = pre_hi ? pre_lo : alo;
-      t.f8 = f8 ? 1 : 0;
-      t.w_blob = f8 ? (upsample ? net->tcw_up8[wname + ".weight"].p : net->tcw8[wname + ".weight"].p)
-                    : (upsample ? net->tcw_up[wname + ".weight"].p : net->tcw[wname + ".weight"].p);
-      t.bias = P(wname + ".bias");
-      t.res1 = res1; t.res2 = res2; t.y = y; t.out_hi = out_hi; t.out_lo = out_lo; t.gn_partial = gn_partial;
-      t.B = B; t.H = Hin; t.W = Win; t.Cin = Cin; t.Cout = Cout; t.ksize = ksize; t.act = act; t.upsample = upsample;
-      t.stride = stride; t.pair = -1; t.strip = -1;
-      const int u = upsample ? 2 : 1;
-      const int Ho = stride == 2 ? (Hin - 1) / 2 + 1 : Hin * u, Wo = stride == 2 ? (Win - 1) / 2 + 1 : Win * u;
-      const double flops = 2.0 * B * Ho * (double)Wo * Cout * Cin * ksize * ksize;   // algorithmic (reference) count
-      const int nkb = (upsample ? 4 : ksize * ksize) * (Cin / 64);
-      const int slice = net->tc_slice_kb;        // k-blocks per accumulator drain (default 4 = 256 of K)
-      if ((precise || precise_region) && net->tc_precise && nkb > slice) {
-        // K-sliced accumulation (layers in front of the VQ): every 256 of K the tensor core's truncating accumulator
-        // is folded into an fp32 round-to-nearest running sum held in registers (see femasr_tc_args.slice_kb)
-        t.slice_kb = slice;
-      }
-      run(detail_name("tc_igemm", ksize, Cin, Cout, Hin, Win, upsample, stride, t.slice_kb), flops,
-          [&] { return femasr_tc_igemm(&t, st); });
-    }
+    const femasr_tc_args t = tc_args(d, m, ahi ? ahi : d.a_hi, ahi ? alo : d.a_lo);
+    run(d.name ? d.name : detail_name("tc_igemm", d.k, d.Cin, d.Cout, d.H, d.W, d.upsample, d.stride, t.slice_kb),
+        conv_flops(d), [&] { return femasr_tc_igemm(&t, st); });
     if (alo) ar.release(alo);
     if (ahi) ar.release(ahi);
   }
 
-  // GroupNorm statistics of x folded into scale/shift tables (allocated by the caller)
-  void gn(const std::string& norm, const float* x, float* sc, float* sh, float* scratch, int B, int HW, int C) {
-    if (dry() || !ok()) return;
-    const float *gw = P(norm + ".weight"), *gb = P(norm + ".bias");
-    run("gn_stats", 0.0, [&] { return femasr_gn_stats(x, gw, gb, sc, sh, scratch, B, HW, C, 1e-6f, st); });
-  }
-
   // GroupNorm partial sums produced by a tensor-core conv epilogue (see femasr_tc_args.gn_partial)
   struct Stats { float* partial = nullptr; int rows = 0; };
-  // for the tensor-core conv [B,H,W,Cin] -> Cout (H,W: conv-input size, low-res if upsample) that will produce them
-  Stats alloc_stats(int B, int H, int W, int Cin, int Cout, int upsample, int stride) {
-    femasr_tc_args t;
-    memset(&t, 0, sizeof(t));
-    t.B = B; t.H = H; t.W = W; t.Cin = Cin; t.Cout = Cout; t.ksize = 3; t.upsample = upsample; t.stride = stride;
-    t.pair = -1; t.strip = -1;
-    t.slice_kb = (precise_region && net->tc_precise && (upsample ? 4 : 9) * (Cin / 64) > net->tc_slice_kb) ? net->tc_slice_kb : 0;
-    Stats st_;
-    st_.rows = femasr_tc_gn_partial_rows(&t);
-    st_.partial = ar.alloc((size_t)B * st_.rows * 32 * 2);
-    return st_;
+  // for the conv d that will produce them (none on the SIMT path)
+  Stats alloc_stats(const ConvDesc& d) {
+    Stats s;
+    if (!use_tc(d)) return s;
+    const femasr_tc_args t = tc_args(d, numerics(d), nullptr, nullptr);
+    s.rows = femasr_tc_gn_partial_rows(&t);
+    s.partial = ar.alloc((size_t)d.B * s.rows * 32 * 2);
+    return s;
   }
-  bool tc_convs(int C) const { return net->cfg.gemm_path == 1 && C % 64 == 0; }
 
   // scale/shift tables for `norm` applied to x: from epilogue partials when available, else a stats pass over x
   void gn_tables(const std::string& norm, const float* x, const Stats& sx, float* sc, float* sh, int B, int HW, int C) {
+    const float *gw = P(norm + ".weight"), *gb = P(norm + ".bias");
     if (sx.partial) {
-      if (dry() || !ok()) return;
-      const float *gw = P(norm + ".weight"), *gb = P(norm + ".bias");
       run("gn_finalize_rows", 0.0, [&] { return femasr_gn_finalize_rows(sx.partial, gw, gb, sc, sh, B, sx.rows, HW, C, 1e-6f, st); });
     } else {
       float* scratch = ar.alloc(femasr_gn_scratch_floats(B, HW, C));
-      gn(norm, x, sc, sh, scratch, B, HW, C);
+      run("gn_stats", 0.0, [&] { return femasr_gn_stats(x, gw, gb, sc, sh, scratch, B, HW, C, 1e-6f, st); });
       ar.release(scratch);
     }
   }
@@ -413,45 +460,36 @@ struct Ctx {
   // output when want_out (for the next ResBlock's first norm), which the caller releases after use.
   Stats resblock(const std::string& p, float* x, int B, int H, int W, int C, const float* extra, Stats sx, bool want_out) {
     const size_t n = (size_t)B * H * W * C;
-    const bool tc = tc_convs(C);
     float* sc = ar.alloc((size_t)B * C);
     float* sh = ar.alloc((size_t)B * C);
     float* t = ar.alloc(n);
     gn_tables(p + ".conv.0.norm", x, sx, sc, sh, B, H * W, C);
     if (sx.partial) ar.release(sx.partial);
-    Stats s1, s2;
-    if (tc) s1 = alloc_stats(B, H, W, C, C, 0, 1);
-    if (tc)
-      conv_tc(p + ".conv.2", x, t, B, H, W, C, C, 3, 0, FEMASR_PRO_GN_SILU, sc, sh, nullptr, nullptr, 0, nullptr, nullptr,
-              nullptr, nullptr, nullptr, nullptr, s1.partial);
-    else
-      conv(p + ".conv.2", x, t, B, H, W, C, C, 3, 1, 0, FEMASR_PRO_GN_SILU, sc, sh, nullptr, nullptr, 0, nullptr, nullptr);
+    ConvDesc c = geom(p + ".conv.2", B, H, W, C, C, 3);
+    c.x = x; c.y = t; c.pro = FEMASR_PRO_GN_SILU; c.pa = sc; c.pb = sh;
+    const Stats s1 = alloc_stats(c);
+    c.gn_partial = s1.partial;
+    conv(c);
     gn_tables(p + ".conv.3.norm", t, s1, sc, sh, B, H * W, C);
     if (s1.partial) ar.release(s1.partial);
-    if (tc && want_out) s2 = alloc_stats(B, H, W, C, C, 0, 1);
-    if (tc)
-      conv_tc(p + ".conv.5", t, x, B, H, W, C, C, 3, 0, FEMASR_PRO_GN_SILU, sc, sh, nullptr, nullptr, 0, x, extra,
-              nullptr, nullptr, nullptr, nullptr, s2.partial);
-    else
-      conv(p + ".conv.5", t, x, B, H, W, C, C, 3, 1, 0, FEMASR_PRO_GN_SILU, sc, sh, nullptr, nullptr, 0, x, extra);
+    c.w = p + ".conv.5"; c.x = t; c.y = x; c.res1 = x; c.res2 = extra;
+    const Stats s2 = want_out ? alloc_stats(c) : Stats{};
+    c.gn_partial = s2.partial;
+    conv(c);
     ar.release(t); ar.release(sh); ar.release(sc);
     return s2;
   }
 
   // nn.Upsample(2) -> conv3x3 -> ResBlock -> ResBlock  (femasr_arch.py:168-180, 195-211); returns new buffer
-  float* up_block(const std::string& pconv, const std::string& prb1, const std::string& prb2, const float* x, int B,
-                  int H, int W, int Cin, int Cout, const float* extra) {
+  float* up_block(const std::string& p, const float* x, int B, int H, int W, int Cin, int Cout, const float* extra) {
     float* y = ar.alloc((size_t)B * 2 * H * 2 * W * Cout);
-    Stats s0;
-    if (tc_convs(Cin) && tc_convs(Cout) && (dry() || net->tcw_up.count(pconv + ".weight"))) {
-      s0 = alloc_stats(B, H, W, Cin, Cout, 1, 1);
-      conv_tc(pconv, x, y, B, H, W, Cin, Cout, 3, 1, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr,
-              nullptr, nullptr, nullptr, nullptr, s0.partial);
-    } else {
-      conv(pconv, x, y, B, H, W, Cin, Cout, 3, 1, 1, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr);
-    }
-    Stats s1 = resblock(prb1, y, B, 2 * H, 2 * W, Cout, nullptr, s0, true);
-    resblock(prb2, y, B, 2 * H, 2 * W, Cout, extra, s1, false);
+    ConvDesc c = geom(p + ".1", B, H, W, Cin, Cout, 3);
+    c.x = x; c.y = y; c.upsample = 1;
+    const Stats s0 = alloc_stats(c);
+    c.gn_partial = s0.partial;
+    conv(c);
+    Stats s1 = resblock(p + ".2", y, B, 2 * H, 2 * W, Cout, nullptr, s0, true);
+    resblock(p + ".3", y, B, 2 * H, 2 * W, Cout, extra, s1, false);
     return y;
   }
 
@@ -465,78 +503,56 @@ struct Ctx {
     float* hid = ar.alloc(M * 4 * C);
     float* mu = ar.alloc(M);
     float* rs = ar.alloc(M);
-    const bool tc = net->cfg.gemm_path == 1 && (dry() || net->tcw.count(p + ".swin_blks.0.conv.weight") != 0);
+    const bool tc = net->cfg.gemm_path == 1;
     for (int r = 0; r < 4; ++r) {
       const std::string rp = p + ".swin_blks." + std::to_string(r);
       for (int b = 0; b < 6; ++b) {
         const std::string bp = rp + ".residual_group.blocks." + std::to_string(b);
         const float* in = b == 0 ? X : T;
-        const float* rb = P(bp + ".attn.relative_position_bias_table");
+        const std::string rbname = bp + ".attn.relative_position_bias_table";
         const double attn_flops = 2.0 * 2.0 * 64 * C * (double)M;
+        ConvDesc q = geom(bp + ".attn.qkv", B, H, W, C, 3 * C, 1), o = geom(bp + ".attn.proj", B, H, W, C, C, 1);
+        ConvDesc f1 = geom(bp + ".mlp.fc1", B, H, W, C, 4 * C, 1), f2 = geom(bp + ".mlp.fc2", B, H, W, 4 * C, C, 1);
+        q.x = in; q.y = qkv; q.pro = FEMASR_PRO_LN; q.gamma = P(bp + ".norm1.weight"); q.beta = P(bp + ".norm1.bias");
+        o.y = T; o.res1 = in;
+        f1.x = T; f1.pro = FEMASR_PRO_LN; f1.gamma = P(bp + ".norm2.weight"); f1.beta = P(bp + ".norm2.bias");
+        f1.act = FEMASR_ACT_GELU;
+        f2.y = T; f2.res1 = T;
         if (tc) {
           // operands travel between the kernels as split fp16 planes: `ao` and `hid` are reinterpreted as
-          // [hi plane | lo plane] (same byte size as the fp32 tensors they replace)
+          // [hi plane | lo plane] (same byte size as the fp32 tensors they replace); LayerNorm runs in the staging
           __half* ao_hi = reinterpret_cast<__half*>(ao);  __half* ao_lo = ao_hi + M * C;
           __half* hd_hi = reinterpret_cast<__half*>(hid); __half* hd_lo = hd_hi + M * 4 * C;
-          conv_tc(bp + ".attn.qkv", in, qkv, B, H, W, C, 3 * C, 1, 0, FEMASR_PRO_LN, nullptr, nullptr, P(bp + ".norm1.weight"),
-                  P(bp + ".norm1.bias"), 0, nullptr, nullptr);
-          const float* rbm = dry() ? nullptr : net->packed_mma[bp + ".attn.relative_position_bias_table"].p;
+          o.a_hi = ao_hi; o.a_lo = ao_lo; f1.o_hi = hd_hi; f1.o_lo = hd_lo; f2.a_hi = hd_hi; f2.a_lo = hd_lo;
+          conv(q);
+          const float* rbm = D(rbname).relb_mma;
           run("window_attention_mma", attn_flops, [&] {
             return femasr_window_attention_mma(qkv, rbm, nullptr, ao_hi, ao_lo, B, H, W, C, 8, (b & 1) ? 4 : 0, st);
           });
-          conv_tc(bp + ".attn.proj", nullptr, T, B, H, W, C, C, 1, 0, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0,
-                  in, nullptr, ao_hi, ao_lo);
-          conv_tc(bp + ".mlp.fc1", T, nullptr, B, H, W, C, 4 * C, 1, 0, FEMASR_PRO_LN, nullptr, nullptr, P(bp + ".norm2.weight"),
-                  P(bp + ".norm2.bias"), FEMASR_ACT_GELU, nullptr, nullptr, nullptr, nullptr, hd_hi, hd_lo);
-          conv_tc(bp + ".mlp.fc2", nullptr, T, B, H, W, 4 * C, C, 1, 0, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0,
-                  T, nullptr, hd_hi, hd_lo);
+          conv(o); conv(f1); conv(f2);
           continue;
         }
+        q.pa = f1.pa = mu; q.pb = f1.pb = rs; o.x = ao; f1.y = hid; f2.x = hid;
+        const float* rb = P(rbname);
         run("ln_stats", 0.0, [&] { return femasr_ln_stats(in, mu, rs, (int)M, C, 1e-5f, st); });
-        conv(bp + ".attn.qkv", in, qkv, B, H, W, C, 3 * C, 1, 1, 0, FEMASR_PRO_LN, mu, rs, P(bp + ".norm1.weight"),
-             P(bp + ".norm1.bias"), 0, nullptr, nullptr);
+        conv(q);
         run("window_attention", attn_flops,
             [&] { return femasr_window_attention(qkv, rb, ao, B, H, W, C, 8, (b & 1) ? 4 : 0, st); });
-        conv(bp + ".attn.proj", ao, T, B, H, W, C, C, 1, 1, 0, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0, in, nullptr);
+        conv(o);
         run("ln_stats", 0.0, [&] { return femasr_ln_stats(T, mu, rs, (int)M, C, 1e-5f, st); });
-        conv(bp + ".mlp.fc1", T, hid, B, H, W, C, 4 * C, 1, 1, 0, FEMASR_PRO_LN, mu, rs, P(bp + ".norm2.weight"),
-             P(bp + ".norm2.bias"), FEMASR_ACT_GELU, nullptr, nullptr);
-        conv(bp + ".mlp.fc2", hid, T, B, H, W, 4 * C, C, 1, 1, 0, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0, T, nullptr);
+        conv(f1); conv(f2);
       }
-      conv(rp + ".conv", T, X, B, H, W, C, C, 3, 1, 0, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0, X, nullptr);
+      ConvDesc c = geom(rp + ".conv", B, H, W, C, C, 3);
+      c.x = T; c.y = X; c.res1 = X;
+      conv(c);
     }
     ar.release(rs); ar.release(mu); ar.release(hid); ar.release(ao); ar.release(qkv); ar.release(T);
-  }
-
-  // One GEMM of the semantic branch with the ReLU epilogue (bias, then ReLU): the 3-product split-fp16 wgmma GEMM in one
-  // pass (no K slices, no F8) on gemm_path 1, the fp32 SIMT GEMM on gemm_path 0.  wkey: the packed weight's key.
-  void sem_gemm(const char* name, const std::string& wname, const std::string& wkey, const void* ahi, const void* alo,
-                const float* ax, float* y, void* ohi, void* olo, int B, int H, int W, int Cin, int Cout, int ksize,
-                double flops) {
-    if (dry() || !ok()) return;
-    if (net->cfg.gemm_path == 1) {
-      auto it = net->tcw.find(wkey);
-      if (it == net->tcw.end()) { check(fail(FEMASR_ERR_STATE, "parameter not set: " + wname + ".weight")); return; }
-      femasr_tc_args t;
-      memset(&t, 0, sizeof(t));
-      t.a_hi = ahi; t.a_lo = alo; t.w_blob = it->second.p; t.bias = P(wname + ".bias");
-      t.y = y; t.out_hi = ohi; t.out_lo = olo;
-      t.B = B; t.H = H; t.W = W; t.Cin = Cin; t.Cout = Cout; t.ksize = ksize; t.act = FEMASR_ACT_RELU;
-      t.stride = 1; t.pair = -1; t.strip = -1; t.slice_kb = net->sem_slice_kb;
-      run(name, flops, [&] { return femasr_tc_igemm(&t, st); });
-    } else {
-      femasr_igemm_args a;
-      memset(&a, 0, sizeof(a));
-      a.x = ax; a.w = P(wkey); a.bias = P(wname + ".bias"); a.y = y;
-      a.B = B; a.Hin = H; a.Win = W; a.Cin = Cin; a.Cout = Cout; a.ksize = ksize; a.stride = 1; a.act = FEMASR_ACT_RELU;
-      if (!ok()) return;
-      run(name, flops, [&] { return femasr_igemm_simt(&a, st); });
-    }
   }
 
   // vgg_feat = relu4_4((x - mean) / std) (femasr_arch.py:318-320).  Runs before the encoder: relu4_4 is allocated first
   // and every full-resolution VGG buffer is released before the encoder's peak.  gemm_path 1 hands the activations from
   // conv to conv as split fp16 planes; the pools read fp32 (pooling before the split) and write the next conv's planes.
+  // Every conv is bias + ReLU: the 3-product split-fp16 wgmma GEMM on gemm_path 1, the fp32 SIMT GEMM on gemm_path 0.
   void semantic_vgg(const float* x_nchw, int B, int H, int W) {
     const bool tc = net->cfg.gemm_path == 1;
     const std::string pre = "vgg_feat_extractor.vgg_net.";
@@ -573,12 +589,11 @@ struct Ctx {
       float* y = last ? vgg_feat : (to_f32 ? ar.alloc(n) : nullptr);
       float *ohi = nullptr, *olo = nullptr;
       if (!to_f32) { ohi = ar.alloc((n + 1) / 2); olo = ar.alloc((n + 1) / 2); }
-      const std::string wn = pre + VGG_CONVS[i];
-      const double flops = 2.0 * B * h * (double)w * co * (i == 0 ? 27 : 9 * c);   // algorithmic (27 MACs for conv1_1)
-      if (i == 0)       // conv1_1: 1x1 GEMM over the K = 27 -> 64 im2col rows
-        sem_gemm("vgg_conv", wn, wn + ".weight#im2col", ahi, alo, af, y, ohi, olo, B, h, w, 64, co, 1, flops);
-      else
-        sem_gemm("vgg_conv", wn, wn + ".weight", ahi, alo, af, y, ohi, olo, B, h, w, c, co, 3, flops);
+      // conv1_1: 1x1 GEMM over the K = 27 -> 64 im2col rows (27 algorithmic MACs)
+      ConvDesc g = geom(pre + VGG_CONVS[i], B, h, w, i == 0 ? 64 : c, co, i == 0 ? 1 : 3);
+      g.name = "vgg_conv"; g.semantic = true; g.im2col = i == 0; g.macs = i == 0 ? 27 : 0; g.act = FEMASR_ACT_RELU;
+      g.x = af; g.a_hi = ahi; g.a_lo = alo; g.y = y; g.o_hi = ohi; g.o_lo = olo;
+      conv(g);
       if (tc) { ar.release(alo); ar.release(ahi); ahi = ohi; alo = olo; }
       else { ar.release(af); af = y; }
       if (to_f32 && !last) f = y;
@@ -600,14 +615,13 @@ struct Ctx {
       zhi = ar.alloc(N * 256); zlo = ar.alloc(N * 256);
       run("tc_prepare", 0.0, [&] { return femasr_tc_prepare(zq, zhi, zlo, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, B, hh, ww, 512, 0, 0.f, st); });
     }
-    sem_gemm("semantic_conv", "conv_semantic.0", "conv_semantic.0.weight", zhi, zlo, zq, s, nullptr, nullptr, B, hh, ww,
-             512, 512, 1, 2.0 * N * 512 * 512);
+    ConvDesc g = geom("conv_semantic.0", B, hh, ww, 512, 512, 1);
+    g.name = "semantic_conv"; g.semantic = true; g.act = FEMASR_ACT_RELU; g.x = zq; g.a_hi = zhi; g.a_lo = zlo; g.y = s;
+    conv(g);
     tap("semantic", s, N * 512);
-    if (!dry() && ok()) {
-      const float* v = vgg_feat;
-      run("semantic_mse", 0.0, [&] { return femasr_sq_diff_rows(s, v, rows, (int)N, 512, st); });
-      run("semantic_mse", 0.0, [&] { return femasr_sum_scaled(rows, sem_loss, N, 1.0 / ((double)N * 512), st); });
-    }
+    const float* v = vgg_feat;
+    run("semantic_mse", 0.0, [&] { return femasr_sq_diff_rows(s, v, rows, (int)N, 512, st); });
+    run("semantic_mse", 0.0, [&] { return femasr_sum_scaled(rows, sem_loss, N, 1.0 / ((double)N * 512), st); });
     if (tc) { ar.release(zlo); ar.release(zhi); }
     ar.release(rows); ar.release(s);
     ar.release(vgg_feat); vgg_feat = nullptr;
@@ -622,10 +636,12 @@ struct Ctx {
     const size_t N = (size_t)B * hh * ww;
     const int e = cb.e_dim;
     float* z = ar.alloc(N * e);
-    conv("before_quant_group." + ks, src, z, B, hh, ww, Cin, e, 1, 1, 0, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr);
+    ConvDesc bq = geom("before_quant_group." + ks, B, hh, ww, Cin, e, 1);
+    bq.x = src; bq.y = z;
+    conv(bq);
     tap(k == 0 ? "z" : (k == 1 ? "z1" : "z2"), z, N * e);
     const std::string cname = "quantize_group." + ks + ".embedding.weight";
-    const bool fused = net->cfg.gemm_path == 1 && net->vq_fused && (dry() || net->tcw.count(cname) != 0);
+    const bool fused = has(cname, FORM_TC);
     // fused: tensor-core distances + in-kernel top-4 (no [N, n_e] tensor); else the fp32 SIMT product + vq_select
     float *zc = nullptr, *arow = nullptr, *zhi = nullptr, *zlo = nullptr, *cand = nullptr;
     if (fused) {
@@ -635,7 +651,9 @@ struct Ctx {
       cand = ar.alloc(N * 8);
     } else {
       zc = ar.alloc(N * cb.n_e);
-      conv("quantize_group." + ks + ".embedding", z, zc, B, hh, ww, e, cb.n_e, 1, 1, 0, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr, false);
+      ConvDesc d = geom("quantize_group." + ks + ".embedding", B, hh, ww, e, cb.n_e, 1);
+      d.x = z; d.y = zc; d.bias = false;
+      conv(d);
     }
     float* zq = ar.alloc(N * e);
     float* lrows = ar.alloc(N);
@@ -643,28 +661,26 @@ struct Ctx {
     float *zq_gt = nullptr, *gpart = nullptr;
     const int gtiles = femasr_gram_diff_tiles(e);
     if (gt_loss) { zq_gt = ar.alloc(N * e); gpart = ar.alloc((size_t)B * gtiles); }
-    if (!dry() && ok()) {
-      const float* cbw = net->raw[cname].p;
-      const float* esq = net->esq[cname].p;
-      if (fused) {
-        const void* cbt = net->tcw[cname].p;
-        run("vq_row_sumsq", 0.0, [&] { return femasr_row_sumsq(z, arow, (int)N, e, st); });
-        run("tc_prepare", 0.0, [&] { return femasr_tc_prepare(z, zhi, zlo, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, B, hh, ww, e, 0, 0.f, st); });
-        run("vq_match_tc", 2.0 * (double)N * cb.n_e * e, [&] { return femasr_vq_match_tc(zhi, zlo, cbt, arow, esq, cand, (int)N, cb.n_e, e, st); });
-        run("vq_finish", 0.0, [&] { return femasr_vq_finish(z, arow, cand, cbw, esq, indices, zq, lrows, nullptr, (int)N, cb.n_e, e, st); });
-      } else {
-        run("vq_select", 0.0, [&] { return femasr_vq_select(z, zc, cbw, esq, indices, zq, lrows, (int)N, cb.n_e, e, 0, st); });
-      }
-      if (cb_loss && !gt_loss) {
-        const double s = 1.25 / ((double)N * e);         // q_latent + 0.25 * e_latent, :92
-        run("sum_scaled", 0.0, [&] { return k == 0 ? femasr_sum_scaled(lrows, cb_loss, N, s, st) : femasr_sum_scaled_add(lrows, cb_loss, N, s, st); });
-      } else if (cb_loss) {
-        run("vq_gt_rows", 0.0, [&] { return femasr_vq_gt_rows(z, cbw, gt, zq_gt, lrows, (int)N, cb.n_e, e, st); });
-        const double s = 0.25 / ((double)N * e);         // beta * mean((z_q_gt - z)^2), :87
-        run("sum_scaled", 0.0, [&] { return k == 0 ? femasr_sum_scaled(lrows, cb_loss, N, s, st) : femasr_sum_scaled_add(lrows, cb_loss, N, s, st); });
-        run("gram_diff", 4.0 * B * (double)hh * ww * e * e, [&] { return femasr_gram_diff(z, zq_gt, gpart, B, hh * ww, e, st); });
-        run("sum_scaled", 0.0, [&] { return femasr_sum_scaled_add(gpart, cb_loss, (size_t)B * gtiles, 1.0 / ((double)B * e * e), st); });
-      }
+    const DevParam& cbd = D(cname);
+    const float *cbw = cbd.raw, *esq = cbd.esq;
+    if (fused) {
+      const void* cbt = cbd.tc;
+      run("vq_row_sumsq", 0.0, [&] { return femasr_row_sumsq(z, arow, (int)N, e, st); });
+      run("tc_prepare", 0.0, [&] { return femasr_tc_prepare(z, zhi, zlo, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, B, hh, ww, e, 0, 0.f, st); });
+      run("vq_match_tc", 2.0 * (double)N * cb.n_e * e, [&] { return femasr_vq_match_tc(zhi, zlo, cbt, arow, esq, cand, (int)N, cb.n_e, e, st); });
+      run("vq_finish", 0.0, [&] { return femasr_vq_finish(z, arow, cand, cbw, esq, indices, zq, lrows, nullptr, (int)N, cb.n_e, e, st); });
+    } else {
+      run("vq_select", 0.0, [&] { return femasr_vq_select(z, zc, cbw, esq, indices, zq, lrows, (int)N, cb.n_e, e, 0, st); });
+    }
+    if (cb_loss && !gt_loss) {
+      const double s = 1.25 / ((double)N * e);         // q_latent + 0.25 * e_latent, :92
+      run("sum_scaled", 0.0, [&] { return k == 0 ? femasr_sum_scaled(lrows, cb_loss, N, s, st) : femasr_sum_scaled_add(lrows, cb_loss, N, s, st); });
+    } else if (cb_loss) {
+      run("vq_gt_rows", 0.0, [&] { return femasr_vq_gt_rows(z, cbw, gt, zq_gt, lrows, (int)N, cb.n_e, e, st); });
+      const double s = 0.25 / ((double)N * e);         // beta * mean((z_q_gt - z)^2), :87
+      run("sum_scaled", 0.0, [&] { return k == 0 ? femasr_sum_scaled(lrows, cb_loss, N, s, st) : femasr_sum_scaled_add(lrows, cb_loss, N, s, st); });
+      run("gram_diff", 4.0 * B * (double)hh * ww * e * e, [&] { return femasr_gram_diff(z, zq_gt, gpart, B, hh * ww, e, st); });
+      run("sum_scaled", 0.0, [&] { return femasr_sum_scaled_add(gpart, cb_loss, (size_t)B * gtiles, 1.0 / ((double)B * e * e), st); });
     }
     if (gt_loss) { ar.release(gpart); ar.release(zq_gt); }
     ar.release(lrows);
@@ -685,7 +701,6 @@ struct Ctx {
     float* prev_q = nullptr; int pq_h = 0, pq_w = 0, pq_e = 0;   // previous z_quant (:358)
     float* prev_z = nullptr;
     size_t idx_off = 0;
-    int Cprev = 0;                            // channels of t
     for (int i = 0; i < 3; ++i) {
       const int hh = h << i, ww = w << i, ch = chan(32 << i), co = chan(64 << i);
       const int k = zq0_given ? (i == 0 ? 0 : -1) : net->level_cb[i];
@@ -701,8 +716,7 @@ struct Ctx {
           int Cin = ch;
           if (t) {                            // cat(enc_feats[i], prev_dec_feat), :332-333
             cat = ar.alloc(N * 2 * ch);
-            if (!dry() && ok())
-              run("concat_channels", 0.0, [&] { return femasr_concat_channels(feats[i], ch, t, hh, ww, ch, cat, B, hh, ww, st); });
+            run("concat_channels", 0.0, [&] { return femasr_concat_channels(feats[i], ch, t, hh, ww, ch, cat, B, hh, ww, st); });
             ar.release(t); t = nullptr;
             src = cat; Cin = 2 * ch;
           }
@@ -719,13 +733,13 @@ struct Ctx {
         if (prev_q) {                         // CombineQuantBlock: cat(z_quant, interpolate(prev_quant)), fema_utils.py:92-99
           cat2 = ar.alloc(N * (cb.e_dim + pq_e));
           const float* a0 = aq; const int pe = pq_e, ph = pq_h, pw = pq_w; const float* pq = prev_q;
-          if (!dry() && ok())
-            run("concat_channels", 0.0, [&] { return femasr_concat_channels(a0, cb.e_dim, pq, ph, pw, pe, cat2, B, hh, ww, st); });
+          run("concat_channels", 0.0, [&] { return femasr_concat_channels(a0, cb.e_dim, pq, ph, pw, pe, cat2, B, hh, ww, st); });
           aq = cat2; e_in += pq_e;
         }
         t = ar.alloc(N * ch);
-        conv("after_quant_group." + std::to_string(k) + ".conv", aq, t, B, hh, ww, e_in, ch, 3, 1, 0, FEMASR_PRO_NONE,
-             nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr);
+        ConvDesc c = geom("after_quant_group." + std::to_string(k) + ".conv", B, hh, ww, e_in, ch, 3);
+        c.x = aq; c.y = t;
+        conv(c);
         if (k == 0) tap("after_quant", t, N * ch);
         if (cat2) ar.release(cat2);
         if (prev_q) { ar.release(prev_q); ar.release(prev_z); }
@@ -734,24 +748,20 @@ struct Ctx {
           pq_h = hh; pq_w = ww; pq_e = cb.e_dim;
         }
       }
-      (void)Cprev;
       // the skip add of the NEXT level (x = x + enc_feats[i+1], :361-362) rides on this block's last epilogue
       const bool next_quant = i + 1 < 3 && !zq0_given && net->level_cb[i + 1] >= 0;
       const float* extra = (i + 1 < 3 && !zq0_given && lq && cfg.use_residual && !next_quant) ? feats[i + 1] : nullptr;
-      const std::string b = "decoder_group." + std::to_string(i) + ".block";
-      float* nt = up_block(b + ".1", b + ".2", b + ".3", t, B, hh, ww, ch, co, extra);
+      float* nt = up_block("decoder_group." + std::to_string(i) + ".block", t, B, hh, ww, ch, co, extra);
       ar.release(t);
       t = nt;
       tap(i == 0 ? "dec0" : (i == 1 ? "dec1" : "dec2"), t, (size_t)B * 2 * hh * 2 * ww * co);
     }
     if (prev_q) { ar.release(prev_q); ar.release(prev_z); }
-    {
-      const float *ow = P("out_conv.weight"), *ob = P("out_conv.bias");
-      const float* d2 = t;
-      run("out_conv", 2.0 * 9 * 64 * 3 * (double)B * 64 * h * w,
-          [&] { return net->cfg.gemm_path == 1 && net->oc_mma ? femasr_out_conv3x3_mma(d2, ow, ob, y_nchw, B, 8 * h, 8 * w, 64, st)
-                                                               : femasr_out_conv3x3(d2, ow, ob, y_nchw, B, 8 * h, 8 * w, 64, st); });
-    }
+    const float *ow = P("out_conv.weight"), *ob = P("out_conv.bias");
+    const float* d2 = t;
+    run("out_conv", 2.0 * 9 * 64 * 3 * (double)B * 64 * h * w,
+        [&] { return net->cfg.gemm_path == 1 ? femasr_out_conv3x3_mma(d2, ow, ob, y_nchw, B, 8 * h, 8 * w, 64, st)
+                                             : femasr_out_conv3x3(d2, ow, ob, y_nchw, B, 8 * h, 8 * w, 64, st); });
     ar.release(t);
   }
 
@@ -761,45 +771,33 @@ struct Ctx {
     const std::string enc = "multiscale_encoder";
     int c = chan(256 / cfg.scale_factor);
     int h = H - 1, w = W - 1;
-    const bool tc = tc_convs(c);
+    const bool tc = cfg.gemm_path == 1;
     if (sem_loss) semantic_vgg(x_nchw, B, H, W);
     precise_region = true;
     const float *iw = P(enc + ".in_conv.weight"), *ib = P(enc + ".in_conv.bias");
-    const double in_flops = 2.0 * 16 * cfg.in_channel * c * (double)B * h * w;
-    const bool want_in_tap = net->taps.count("in_conv") && net->taps["in_conv"].dst;
     float* cur = nullptr;                 // fp32 in_conv output (SIMT path, or when its tap is requested)
     float* in_hi = nullptr; float* in_lo = nullptr;   // tensor-core path: in_conv writes the split operand planes directly
     const size_t in_elems = (size_t)B * h * w * c;
-    if (!tc || want_in_tap) {     // identical in the dry (sizing) run and the real run: taps are registered first
+    if (!tc || tapped("in_conv")) {       // identical in the sizing run and the real run: taps are registered first
       cur = ar.alloc(in_elems);
       const int c0 = c;
-      if (!tc || want_in_tap)
-        run("in_conv", in_flops, [&] { return femasr_in_conv4x4(x_nchw, iw, ib, cur, B, cfg.in_channel, H, W, c0, st); });
+      run("in_conv", 2.0 * 16 * cfg.in_channel * c * (double)B * h * w,
+          [&] { return femasr_in_conv4x4(x_nchw, iw, ib, cur, B, cfg.in_channel, H, W, c0, st); });
       tap("in_conv", cur, in_elems);
     }
     if (tc) {
+      // K = 48 (-> 64) GEMM over im2col rows on the tensor cores, writing the down conv's split planes
       in_hi = ar.alloc((in_elems + 1) / 2);
       in_lo = ar.alloc((in_elems + 1) / 2);
-      const int c0 = c;
-      const std::string wkey = enc + ".in_conv.weight#im2col";
-      if (net->in_conv_tc && (dry() || net->tcw.count(wkey))) {
-        // K = 48 (-> 64) GEMM over im2col rows on the tensor cores, writing the down conv's split planes
-        const size_t rows = (size_t)B * h * w;
-        float* ic_hi = ar.alloc(rows * 64 / 2);
-        float* ic_lo = ar.alloc(rows * 64 / 2);
-        run("in_conv_im2col", 0.0, [&] { return femasr_in_conv_im2col(x_nchw, ic_hi, ic_lo, B, cfg.in_channel, H, W, st); });
-        if (!dry() && ok()) {
-          femasr_tc_args t;
-          memset(&t, 0, sizeof(t));
-          t.a_hi = ic_hi; t.a_lo = ic_lo; t.w_blob = net->tcw[wkey].p; t.bias = ib;
-          t.out_hi = in_hi; t.out_lo = in_lo;
-          t.B = B; t.H = h; t.W = w; t.Cin = 64; t.Cout = c0; t.ksize = 1; t.stride = 1; t.pair = -1; t.strip = -1;
-          run("in_conv", in_flops, [&] { return femasr_tc_igemm(&t, st); });
-        }
-        ar.release(ic_lo); ar.release(ic_hi);
-      } else {
-        run("in_conv", in_flops, [&] { return femasr_in_conv4x4_split(x_nchw, iw, ib, in_hi, in_lo, B, cfg.in_channel, H, W, c0, st); });
-      }
+      const size_t rows = (size_t)B * h * w;
+      float* ic_hi = ar.alloc(rows * 64 / 2);
+      float* ic_lo = ar.alloc(rows * 64 / 2);
+      run("in_conv_im2col", 0.0, [&] { return femasr_in_conv_im2col(x_nchw, ic_hi, ic_lo, B, cfg.in_channel, H, W, st); });
+      ConvDesc g = geom(enc + ".in_conv", B, h, w, 64, c, 1);
+      g.name = "in_conv"; g.im2col = true; g.macs = 16 * cfg.in_channel;
+      g.a_hi = ic_hi; g.a_lo = ic_lo; g.o_hi = in_hi; g.o_lo = in_lo;
+      conv(g);
+      ar.release(ic_lo); ar.release(ic_hi);
     }
     // which enc_feats the decoder loop reads: at quantising levels (before_quant input) and, in the LQ stage with
     // use_residual, at the other levels > 0 (skip adds)
@@ -811,14 +809,12 @@ struct Ctx {
       const std::string b = enc + ".blocks." + std::to_string(i);
       const int ho = (h + 2 - 3) / 2 + 1, wo = (w + 2 - 3) / 2 + 1, co = chan((256 / cfg.scale_factor) >> (i + 1));
       float* nxt = ar.alloc((size_t)B * ho * wo * co);
-      Stats sd0;
-      if (tc) {
-        sd0 = alloc_stats(B, h, w, c, co, 0, 2);
-        conv_tc(b + ".0", cur, nxt, B, h, w, c, co, 3, 0, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr,
-                i == 0 ? in_hi : nullptr, i == 0 ? in_lo : nullptr, nullptr, nullptr, sd0.partial, 2);
-      } else {
-        conv(b + ".0", cur, nxt, B, h, w, c, co, 3, 2, 0, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr);
-      }
+      ConvDesc g = geom(b + ".0", B, h, w, c, co, 3);
+      g.stride = 2; g.x = cur; g.y = nxt;
+      if (i == 0) { g.a_hi = in_hi; g.a_lo = in_lo; }
+      const Stats sd0 = alloc_stats(g);
+      g.gn_partial = sd0.partial;
+      conv(g);
       if (i == 0 && in_lo) { ar.release(in_lo); ar.release(in_hi); in_lo = in_hi = nullptr; }
       // HQ stage: enc_feats = the down blocks' outputs reversed (:316); block i-1's output is level d-i
       if (cur) { if (net->hq && i > 0 && need[d - i]) feats[d - i] = cur; else ar.release(cur); }
@@ -833,12 +829,11 @@ struct Ctx {
     // the up branches reach the decoder's skip adds (femasr_arch.py:361-362) and, in multi-scale nets, the later quantisers
     precise_region = net->last_q_level >= 1;
     if (!net->hq && (need[1] || need[2])) {
-      const std::string b1 = enc + ".blocks." + std::to_string(d + 1), b2 = enc + ".blocks." + std::to_string(d + 2);
-      feats[1] = up_block(b1 + ".1", b1 + ".2", b1 + ".3", cur, B, h, w, 256, 256, nullptr);
+      feats[1] = up_block(enc + ".blocks." + std::to_string(d + 1), cur, B, h, w, 256, 256, nullptr);
       tap("up1", feats[1], (size_t)B * 2 * h * 2 * w * 256);
       if (need[2]) {
         precise_region = net->last_q_level >= 2;
-        feats[2] = up_block(b2 + ".1", b2 + ".2", b2 + ".3", feats[1], B, 2 * h, 2 * w, 256, 128, nullptr);
+        feats[2] = up_block(enc + ".blocks." + std::to_string(d + 2), feats[1], B, 2 * h, 2 * w, 256, 128, nullptr);
         tap("up2", feats[2], (size_t)B * 4 * h * 4 * w * 128);
       }
     }
@@ -851,10 +846,8 @@ struct Ctx {
     const femasr_net::Codebook& cb = net->cbs[0];
     const size_t N = (size_t)B * h * w;
     float* zq = ar.alloc(N * cb.e_dim);
-    if (!dry() && ok()) {
-      const float* cbw = net->raw["quantize_group.0.embedding.weight"].p;
-      run("codebook_gather", 0.0, [&] { return femasr_codebook_gather(idx, cbw, zq, (int)N, cb.n_e, cb.e_dim, st); });
-    }
+    const float* cbw = D("quantize_group.0.embedding.weight").raw;
+    run("codebook_gather", 0.0, [&] { return femasr_codebook_gather(idx, cbw, zq, (int)N, cb.n_e, cb.e_dim, st); });
     const float* none[3] = {nullptr, nullptr, nullptr};
     decode_loop(none, zq, y_nchw, nullptr, nullptr, nullptr, B, h, w);
     ar.release(zq);
@@ -900,12 +893,19 @@ static int workspace_impl(femasr_net* net, int B, int H, int W, bool with_sem, s
   int s = check_geometry(net, B, H, W);
   if (s) return s;
   if (with_sem && (s = check_semantic(net, H, W))) return s;
-  Ctx c; c.net = net; c.st = nullptr; c.ar.dry = true; c.ar.base = reinterpret_cast<char*>(uintptr_t(1) << 40);
+  Ctx c(net, nullptr, 0, nullptr);
   if (with_sem) c.sem_loss = reinterpret_cast<float*>(uintptr_t(8));
   // sized for the gt_indices loss branch too (its scratch is small): one workspace serves forward and forward_gt
   c.forward(nullptr, nullptr, nullptr, nullptr, reinterpret_cast<const int64_t*>(uintptr_t(8)), B, H, W);
-  *bytes = c.ar.peak + 256;
+  *bytes = c.bytes_needed();
   return c.status;
+}
+
+// cudaMalloc on the first set_param of a parameter; later calls repack into the same buffer
+template <class T>
+static int ensure(T** p, size_t bytes) {
+  if (!*p) FEMASR_CUDA(cudaMalloc(reinterpret_cast<void**>(p), bytes));
+  return FEMASR_OK;
 }
 
 }  // namespace femasr
@@ -953,9 +953,7 @@ extern "C" int femasr_net_create(const femasr_net_config* cfg, femasr_net** out)
   n->hq = cfg->scale_factor == 1;
   if (const char* ev = getenv("FEMASR_TC_PRECISE")) n->tc_precise = atoi(ev) != 0;
   if (const char* ev = getenv("FEMASR_FAST_SILU")) n->fast_silu = atoi(ev) != 0;
-  if (const char* ev = getenv("FEMASR_OUTCONV_MMA")) n->oc_mma = atoi(ev) != 0;
   if (const char* ev = getenv("FEMASR_VQ_FUSED")) n->vq_fused = atoi(ev) != 0;
-  if (const char* ev = getenv("FEMASR_IN_CONV_TC")) n->in_conv_tc = atoi(ev) != 0;
   if (const char* ev = getenv("FEMASR_F8_CROSS")) n->f8_cross = atoi(ev) != 0;
   if (const char* ev = getenv("FEMASR_TC_SLICE_KB")) n->tc_slice_kb = std::max(1, atoi(ev));
   if (const char* ev = getenv("FEMASR_SEM_SLICE_KB")) n->sem_slice_kb = std::max(0, atoi(ev));
@@ -969,12 +967,13 @@ extern "C" void femasr_net_destroy(femasr_net* net) { delete net; }
 extern "C" int femasr_net_enable_semantic(femasr_net* net) {
   FEMASR_CHECK_ARG(net, "enable_semantic: null");
   if (net->semantic) return FEMASR_OK;
-  if (!net->raw.empty()) return fail(FEMASR_ERR_STATE, "enable_semantic: call it before the first set_param");
+  if (!net->dev.empty()) return fail(FEMASR_ERR_STATE, "enable_semantic: call it before the first set_param");
   add_semantic(net);
   net->semantic = true;
   return FEMASR_OK;
 }
 
+// Copies the parameter and packs every device form its ParamInfo lists.
 extern "C" int femasr_net_set_param(femasr_net* net, const char* name, const float* data, size_t numel, int on_device,
                                     void* stream) {
   FEMASR_CHECK_ARG(net && name && data, "set_param: null pointer");
@@ -983,112 +982,45 @@ extern "C" int femasr_net_set_param(femasr_net* net, const char* name, const flo
   const ParamInfo& pi = it->second;
   if (pi.numel != numel) return fail(FEMASR_ERR_ARG, std::string("set_param: wrong size for ") + name);
   cudaStream_t st = as_stream(stream);
-  DevBuf& rb = net->raw[name];
-  if (!rb.p) { FEMASR_CUDA(cudaMalloc(&rb.p, numel * sizeof(float))); rb.n = numel; }
-  FEMASR_CUDA(cudaMemcpyAsync(rb.p, data, numel * sizeof(float), on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+  DevParam& d = net->dev[name];
+  int s = ensure(&d.raw, numel * sizeof(float));
+  if (s) return s;
+  FEMASR_CUDA(cudaMemcpyAsync(d.raw, data, numel * sizeof(float), on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
   if (!on_device) FEMASR_CUDA(cudaStreamSynchronize(st));   // the host buffer may be pageable / freed by the caller
-  std::string key(name);
-  if (pi.kind == 1) {
-    DevBuf& pb = net->packed[key];
-    if (!pb.p) { FEMASR_CUDA(cudaMalloc(&pb.p, numel * sizeof(float))); pb.n = numel; }
-    int s = femasr_pack_weight(rb.p, pb.p, pi.Cout, pi.Cin, pi.k, pi.k, st);
+  const unsigned f = pi.forms;
+  const int co = pi.Cout, ci = pi.Cin, k = pi.k;
+  const size_t tcb = femasr_tc_weight_bytes(co, ci, k, k), upb = femasr_tc_weight_bytes(4 * co, ci, 2, 2);
+  if ((f & FORM_KMAJOR) && ((s = ensure(&d.packed, numel * sizeof(float))) || (s = femasr_pack_weight(d.raw, d.packed, co, ci, k, k, st))))
+    return s;
+  if (f & FORM_IM2COL) {
+    // the im2col GEMM's weight: the [Cout][64] zero-padded matrix (K = 48 for in_conv, 27 for VGG conv1_1), packed
+    // for this net's GEMM path
+    const bool tc = net->cfg.gemm_path == 1;
+    float* tmp = nullptr;
+    FEMASR_CUDA(cudaMallocAsync(&tmp, (size_t)co * 64 * sizeof(float), st));
+    s = k == 4 ? femasr_in_conv_pad_weight(d.raw, tmp, co, st) : femasr_vgg_pad_weight(d.raw, tmp, co, st);
+    if (!s) s = ensure(&d.im2col, tc ? femasr_tc_weight_bytes(co, 64, 1, 1) : (size_t)co * 64 * sizeof(float));
+    if (!s) s = tc ? femasr_tc_pack_weight(tmp, d.im2col, co, 64, 1, 1, st)
+                   : femasr_pack_weight(tmp, static_cast<float*>(d.im2col), co, 64, 1, 1, st);
+    cudaFreeAsync(tmp, st);
     if (s) return s;
-    const bool vgg = key.rfind("vgg_feat_extractor.", 0) == 0;
-    if (vgg && pi.Cin == 3) {
-      // VGG conv1_1 as a K = 27 -> 64 GEMM over normalised im2col rows: [Cout][64] padded matrix -> K-major fp32
-      // (gemm_path 0) or split-fp16 blob (gemm_path 1)
-      float* tmp = nullptr;
-      FEMASR_CUDA(cudaMallocAsync(&tmp, (size_t)pi.Cout * 64 * sizeof(float), st));
-      s = femasr_vgg_pad_weight(rb.p, tmp, pi.Cout, st);
-      if (!s && net->cfg.gemm_path == 1) {
-        DevBuf& tb = net->tcw[key + "#im2col"];
-        const size_t bytes = femasr_tc_weight_bytes(pi.Cout, 64, 1, 1);
-        if (!tb.p) { if (cudaMalloc(&tb.p, bytes) != cudaSuccess) s = fail(FEMASR_ERR_CUDA, "cudaMalloc failed"); tb.n = bytes / sizeof(float); }
-        if (!s) s = femasr_tc_pack_weight(tmp, tb.p, pi.Cout, 64, 1, 1, st);
-      } else if (!s) {
-        DevBuf& kb = net->packed[key + "#im2col"];
-        if (!kb.p) { if (cudaMalloc(&kb.p, (size_t)pi.Cout * 64 * sizeof(float)) != cudaSuccess) s = fail(FEMASR_ERR_CUDA, "cudaMalloc failed"); kb.n = (size_t)pi.Cout * 64; }
-        if (!s) s = femasr_pack_weight(tmp, kb.p, pi.Cout, 64, 1, 1, st);
-      }
-      cudaFreeAsync(tmp, st);
-      return s;
-    }
-    if (net->cfg.gemm_path == 1 && net->in_conv_tc && pi.k == 4 && pi.Cin == 3 && pi.Cout % 64 == 0) {
-      // in_conv as a K = 48 -> 64 tensor-core GEMM over im2col rows: [Cout][64] padded matrix -> split-fp16 blob
-      float* tmp = nullptr;
-      FEMASR_CUDA(cudaMallocAsync(&tmp, (size_t)pi.Cout * 64 * sizeof(float), st));
-      s = femasr_in_conv_pad_weight(rb.p, tmp, pi.Cout, st);
-      DevBuf& tb = net->tcw[key + "#im2col"];
-      const size_t bytes = femasr_tc_weight_bytes(pi.Cout, 64, 1, 1);
-      if (!s && !tb.p) { if (cudaMalloc(&tb.p, bytes) != cudaSuccess) s = fail(FEMASR_ERR_CUDA, "cudaMalloc failed"); tb.n = bytes / sizeof(float); }
-      if (!s) s = femasr_tc_pack_weight(tmp, tb.p, pi.Cout, 64, 1, 1, st);
-      cudaFreeAsync(tmp, st);
-      return s;
-    }
-    if (net->cfg.gemm_path == 1 && (pi.k == 1 || pi.k == 3) && pi.Cin % 64 == 0 && pi.Cout % 64 == 0) {
-      DevBuf& tb = net->tcw[key];
-      const size_t bytes = femasr_tc_weight_bytes(pi.Cout, pi.Cin, pi.k, pi.k);
-      if (!tb.p) { FEMASR_CUDA(cudaMalloc(&tb.p, bytes)); tb.n = bytes / sizeof(float); }
-      s = femasr_tc_pack_weight(rb.p, tb.p, pi.Cout, pi.Cin, pi.k, pi.k, st);
-      if (s) return s;
-      if (net->f8_cross && pi.k == 3 && !vgg) {      // a 3x3 conv may run behind the VQ (the VGG convs never use F8): keep the F8 packing next to the fp16 one
-        DevBuf& t8 = net->tcw8[key];
-        if (!t8.p) { FEMASR_CUDA(cudaMalloc(&t8.p, bytes)); t8.n = bytes / sizeof(float); }
-        s = femasr_tc_pack_weight_f8(rb.p, t8.p, pi.Cout, pi.Cin, pi.k, pi.k, st);
-        if (s) return s;
-      }
-      // the five nearest-x2 -> conv3x3 sites (femasr_arch.py:172-173, 202-203) also get sub-pixel phase filters
-      const std::string up1 = "multiscale_encoder.blocks." + std::to_string(net->depth + 1) + ".1.weight";
-      const std::string up2 = "multiscale_encoder.blocks." + std::to_string(net->depth + 2) + ".1.weight";
-      const bool is_up = pi.k == 3 && (key == up1 || key == up2 || (key.rfind("decoder_group.", 0) == 0 &&
-                                        key.size() > 15 && key.compare(key.size() - 15, 15, ".block.1.weight") == 0));
-      if (is_up) {
-        DevBuf& ub = net->tcw_up[key];
-        const size_t ubytes = femasr_tc_weight_bytes(4 * pi.Cout, pi.Cin, 2, 2);
-        if (!ub.p) { FEMASR_CUDA(cudaMalloc(&ub.p, ubytes)); ub.n = ubytes / sizeof(float); }
-        s = femasr_tc_pack_weight_up2(rb.p, ub.p, pi.Cout, pi.Cin, st);
-        if (s || !net->f8_cross) return s;
-        DevBuf& u8 = net->tcw_up8[key];
-        if (!u8.p) { FEMASR_CUDA(cudaMalloc(&u8.p, ubytes)); u8.n = ubytes / sizeof(float); }
-        return femasr_tc_pack_weight_up2_f8(rb.p, u8.p, pi.Cout, pi.Cin, st);
-      }
-      return FEMASR_OK;
-    }
-    return FEMASR_OK;
   }
-  if (pi.kind == 2) {
-    DevBuf& pb = net->packed[key];
-    if (!pb.p) { FEMASR_CUDA(cudaMalloc(&pb.p, 8 * 64 * 64 * sizeof(float))); pb.n = 8 * 64 * 64; }
-    DevBuf& mb = net->packed_mma[key];
-    if (!mb.p) { FEMASR_CUDA(cudaMalloc(&mb.p, 8 * 64 * 64 * sizeof(float))); mb.n = 8 * 64 * 64; }
-    int s = femasr_expand_rel_bias_mma(rb.p, mb.p, 8, st);
-    if (s) return s;
-    return femasr_expand_rel_bias(rb.p, pb.p, 8, st);
-  }
-  if (pi.kind == 3) {
-    DevBuf& pb = net->packed[key];     // codebook^T as a GEMM operand [e_dim][n_e]
-    if (!pb.p) { FEMASR_CUDA(cudaMalloc(&pb.p, numel * sizeof(float))); pb.n = numel; }
-    int s = femasr_pack_weight(rb.p, pb.p, pi.Cout, pi.Cin, 1, 1, st);
-    if (s) return s;
-    DevBuf& eb = net->esq[key];
-    if (!eb.p) { FEMASR_CUDA(cudaMalloc(&eb.p, pi.Cout * sizeof(float))); eb.n = pi.Cout; }
-    s = femasr_row_sumsq(rb.p, eb.p, pi.Cout, pi.Cin, st);
-    if (s) return s;
-    if (net->cfg.gemm_path == 1 && net->vq_fused) {     // split-fp16 planes of the [n_e, e_dim] embedding: B operand of the fused VQ
-      DevBuf& tb = net->tcw[key];
-      const size_t bytes = femasr_tc_weight_bytes(pi.Cout, pi.Cin, 1, 1);
-      if (!tb.p) { FEMASR_CUDA(cudaMalloc(&tb.p, bytes)); tb.n = bytes / sizeof(float); }
-      return femasr_tc_pack_weight(rb.p, tb.p, pi.Cout, pi.Cin, 1, 1, st);
-    }
-    return FEMASR_OK;
-  }
+  if ((f & FORM_TC) && ((s = ensure(&d.tc, tcb)) || (s = femasr_tc_pack_weight(d.raw, d.tc, co, ci, k, k, st)))) return s;
+  if ((f & FORM_TC8) && ((s = ensure(&d.tc8, tcb)) || (s = femasr_tc_pack_weight_f8(d.raw, d.tc8, co, ci, k, k, st)))) return s;
+  if ((f & FORM_UP) && ((s = ensure(&d.up, upb)) || (s = femasr_tc_pack_weight_up2(d.raw, d.up, co, ci, st)))) return s;
+  if ((f & FORM_UP8) && ((s = ensure(&d.up8, upb)) || (s = femasr_tc_pack_weight_up2_f8(d.raw, d.up8, co, ci, st)))) return s;
+  if ((f & FORM_RELB) &&
+      ((s = ensure(&d.packed, 8 * 64 * 64 * sizeof(float))) || (s = ensure(&d.relb_mma, 8 * 64 * 64 * sizeof(float))) ||
+       (s = femasr_expand_rel_bias_mma(d.raw, d.relb_mma, 8, st)) || (s = femasr_expand_rel_bias(d.raw, d.packed, 8, st))))
+    return s;
+  if ((f & FORM_ESQ) && ((s = ensure(&d.esq, co * sizeof(float))) || (s = femasr_row_sumsq(d.raw, d.esq, co, ci, st)))) return s;
   return FEMASR_OK;
 }
 
 extern "C" int femasr_net_params_complete(femasr_net* net) {
   FEMASR_CHECK_ARG(net, "params_complete: null");
   for (auto& kv : net->spec)
-    if (net->raw.find(kv.first) == net->raw.end()) return fail(FEMASR_ERR_STATE, "parameter not set: " + kv.first);
+    if (net->dev.find(kv.first) == net->dev.end()) return fail(FEMASR_ERR_STATE, "parameter not set: " + kv.first);
   return FEMASR_OK;
 }
 
@@ -1124,21 +1056,18 @@ extern "C" int femasr_net_forward_sem(femasr_net* net, const float* x, float* y,
   size_t need = 0;
   s = workspace_impl(net, B, H, W, sem_loss != nullptr, &need);
   if (s) return s;
-  const uintptr_t mis = (256 - ((uintptr_t)workspace & 255)) & 255;
   if (workspace_bytes < need) return fail(FEMASR_ERR_STATE, "forward: workspace too small (need " + std::to_string(need) + " bytes)");
-  Ctx c; c.net = net; c.st = as_stream(stream); c.ar.dry = false; c.sem_loss = sem_loss;
-  c.ar.base = reinterpret_cast<char*>(workspace) + mis; c.ar.cap = workspace_bytes - mis;
-  const long l0 = g_launches;
+  Ctx c(net, workspace, workspace_bytes, stream);
+  c.sem_loss = sem_loss;
   c.forward(x, y, indices, cb_loss, gt_indices, B, H, W);
-  net->last_launches = (int)(g_launches - l0);
-  return c.status;
+  return c.finish();
 }
 
 extern "C" int femasr_net_decode_workspace_bytes(femasr_net* net, int B, int h, int w, size_t* bytes) {
   FEMASR_CHECK_ARG(net && bytes && B > 0 && h > 0 && w > 0, "decode_workspace_bytes: bad argument");
-  Ctx c; c.net = net; c.st = nullptr; c.ar.dry = true; c.ar.base = reinterpret_cast<char*>(uintptr_t(1) << 40);
+  Ctx c(net, nullptr, 0, nullptr);
   c.decode_indices(nullptr, nullptr, B, h, w);
-  *bytes = c.ar.peak + 256;
+  *bytes = c.bytes_needed();
   return c.status;
 }
 
@@ -1151,13 +1080,9 @@ extern "C" int femasr_net_decode_indices(femasr_net* net, const int64_t* indices
   s = femasr_net_decode_workspace_bytes(net, B, h, w, &need);
   if (s) return s;
   if (workspace_bytes < need) return fail(FEMASR_ERR_STATE, "decode_indices: workspace too small");
-  const uintptr_t mis = (256 - ((uintptr_t)workspace & 255)) & 255;
-  Ctx c; c.net = net; c.st = as_stream(stream); c.ar.dry = false;
-  c.ar.base = reinterpret_cast<char*>(workspace) + mis; c.ar.cap = workspace_bytes - mis;
-  const long l0 = g_launches;
+  Ctx c(net, workspace, workspace_bytes, stream);
   c.decode_indices(indices, y, B, h, w);
-  net->last_launches = (int)(g_launches - l0);
-  return c.status;
+  return c.finish();
 }
 
 extern "C" int femasr_net_set_tap(femasr_net* net, const char* stage, float* dst, size_t capacity) {
@@ -1208,31 +1133,14 @@ extern "C" const char* femasr_net_profile_json(femasr_net* net) {
   return net->prof_json.c_str();
 }
 
+// The sum of the algorithmic FLOPs the launches of one plain forward report (no taps, no gt_indices, no semantic loss),
+// counted by a sizing run; 0 for a geometry forward rejects.
 extern "C" double femasr_net_flops(femasr_net* net, int B, int H, int W) {
-  if (!net) return 0.0;
-  const int scale = net->cfg.scale_factor, d = net->depth;
-  const double cin = chan(256 / scale);
-  double f = 2.0 * 3 * 16 * cin * (H - 1) * (double)(W - 1);
-  double ch = cin, hh = H, ww = W;
-  for (int i = 0; i < d; ++i) {
-    hh = std::floor(hh / 2); ww = std::floor(ww / 2);
-    const double co = chan((256 / scale) >> (i + 1));
-    f += 2.0 * 9 * ch * co * hh * ww + 4 * 2.0 * 9 * co * co * hh * ww;
-    ch = co;
-  }
-  const double px = hh * ww;
-  const double lin = 2.0 * 256 * (768 + 256 + 1024 + 1024) * px, att = 2 * 2.0 * 64 * 256 * px;
-  if (!net->hq) f += 4 * (6 * (lin + att) + 2.0 * 9 * 256 * 256 * px);
-  for (size_t k = 0; k < net->cbs.size(); ++k) {      // before_quant 1x1, z.E^T, after_quant 3x3 at each codebook's level
-    const femasr_net::Codebook& cb = net->cbs[k];
-    const double m = cb.scale / 32.0, pk = px * m * m, chk = chan(cb.scale), e = cb.e_dim;
-    const double ein = k == 0 ? e : e + net->cbs[k - 1].e_dim;
-    f += 2.0 * (k == 0 ? chk : 2 * chk) * e * pk + 2.0 * cb.n_e * e * pk + 2.0 * 9 * ein * chk * pk;
-  }
-  const double up[2][3] = {{256, 256, 2}, {256, 128, 4}};
-  if (!net->hq) for (auto& u : up) f += (2.0 * 9 * u[0] * u[1] + 4 * 2.0 * 9 * u[1] * u[1]) * px * u[2] * u[2];
-  const double dec[3][3] = {{256, 256, 2}, {256, 128, 4}, {128, 64, 8}};
-  for (auto& u : dec) f += (2.0 * 9 * u[0] * u[1] + 4 * 2.0 * 9 * u[1] * u[1]) * px * u[2] * u[2];
-  f += 2.0 * 9 * 64 * 3 * px * 64;
-  return f * B;
+  if (!net || check_geometry(net, B, H, W)) return 0.0;
+  std::map<std::string, Tap> taps;
+  taps.swap(net->taps);          // a registered in_conv tap adds the fp32 in_conv to the tensor-core plan
+  Ctx c(net, nullptr, 0, nullptr);
+  c.forward(nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W);
+  taps.swap(net->taps);
+  return c.flops;
 }
