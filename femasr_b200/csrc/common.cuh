@@ -110,6 +110,38 @@ __device__ __forceinline__ long pool2_max8(const float* __restrict__ x, long i, 
   return pix * C + cq * 8;
 }
 
+// F.interpolate(scale_factor=2, mode='bilinear', align_corners=False) of 8 consecutive channels: element i of the
+// upsampled NHWC tensor [B,2H,2W,C] in 8-channel units; returns its element offset.  Source index and weights as ATen
+// computes them (src = max(0.5 * (o + 0.5) - 0.5, 0), the far neighbour clamped at the border), then
+// h0 * (w0 * x00 + w1 * x01) + h1 * (w0 * x10 + w1 * x11).
+__device__ __forceinline__ long bilinear2_8(const float* __restrict__ x, long i, int H, int W, int C, float (&v)[8]) {
+  const int c8 = C / 8, Ho = 2 * H, Wo = 2 * W;
+  const int cq = (int)(i % c8);
+  const long pix = i / c8;
+  const int ox = (int)(pix % Wo);
+  const long t = pix / Wo;
+  const int oy = (int)(t % Ho);
+  const long b = t / Ho;
+  const float sy = fmaxf(0.5f * (oy + 0.5f) - 0.5f, 0.f), sx = fmaxf(0.5f * (ox + 0.5f) - 0.5f, 0.f);
+  const int y0 = (int)sy, x0 = (int)sx;
+  const int y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
+  const float h1 = sy - y0, h0 = 1.f - h1, w1 = sx - x0, w0 = 1.f - w1;
+  float a[4][8];
+  const int ys[2] = {y0, y1}, xs[2] = {x0, x1};
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float4* s = reinterpret_cast<const float4*>(x + ((b * H + ys[q >> 1]) * W + xs[q & 1]) * C + cq * 8);
+    const float4 p0 = __ldg(s), p1 = __ldg(s + 1);
+    a[q][0] = p0.x; a[q][1] = p0.y; a[q][2] = p0.z; a[q][3] = p0.w;
+    a[q][4] = p1.x; a[q][5] = p1.y; a[q][6] = p1.z; a[q][7] = p1.w;
+  }
+#pragma unroll
+  for (int k = 0; k < 8; ++k) v[k] = h0 * (w0 * a[0][k] + w1 * a[1][k]) + h1 * (w0 * a[2][k] + w1 * a[3][k]);
+  return pix * C + cq * 8;
+}
+
+__device__ __forceinline__ float lrelu02_f(float v) { return v > 0.f ? v : v * 0.2f; }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -90,6 +90,8 @@ constexpr int OC_CIN = 64, OC_TH = 4, OC_TW = 32, OC_PS = 68;   // pixel stride 
 __constant__ float c_outconv_w[9 * OC_CIN * 3];
 __constant__ float c_outconv_b[4];
 
+// CO output channels (3: out_conv, 1: the discriminator's conv9); the weights use the first 9 * OC_CIN * CO floats
+template <int CO>
 __global__ void __launch_bounds__(OC_TH * OC_TW) out_conv_kernel(const float* __restrict__ x, float* __restrict__ y,
                                                                  int B, int H, int W) {
   extern __shared__ __align__(16) float tile[];      // [(OC_TH+2)][(OC_TW+2)][OC_PS]
@@ -109,27 +111,31 @@ __global__ void __launch_bounds__(OC_TH * OC_TW) out_conv_kernel(const float* __
   __syncthreads();
   const int lx = threadIdx.x % OC_TW, ly = threadIdx.x / OC_TW;
   const int ox = x0 + lx, oy = y0 + ly;
-  float a0 = c_outconv_b[0], a1 = c_outconv_b[1], a2 = c_outconv_b[2];
+  float a[CO];
+#pragma unroll
+  for (int co = 0; co < CO; ++co) a[co] = c_outconv_b[co];
 #pragma unroll 1
   for (int kh = 0; kh < 3; ++kh)
 #pragma unroll
     for (int kw = 0; kw < 3; ++kw) {
       const float* px = &tile[((ly + kh) * TWH + lx + kw) * OC_PS];
-      const float* wt = c_outconv_w + (kh * 3 + kw) * OC_CIN * 3;
+      const float* wt = c_outconv_w + (kh * 3 + kw) * OC_CIN * CO;
 #pragma unroll 4
       for (int c4 = 0; c4 < OC_CIN / 4; ++c4) {
         const float4 v = *reinterpret_cast<const float4*>(px + c4 * 4);
-        const float* wk = wt + c4 * 12;
-        a0 = fmaf(v.x, wk[0], a0); a1 = fmaf(v.x, wk[1], a1); a2 = fmaf(v.x, wk[2], a2);
-        a0 = fmaf(v.y, wk[3], a0); a1 = fmaf(v.y, wk[4], a1); a2 = fmaf(v.y, wk[5], a2);
-        a0 = fmaf(v.z, wk[6], a0); a1 = fmaf(v.z, wk[7], a1); a2 = fmaf(v.z, wk[8], a2);
-        a0 = fmaf(v.w, wk[9], a0); a1 = fmaf(v.w, wk[10], a1); a2 = fmaf(v.w, wk[11], a2);
+        const float vv[4] = {v.x, v.y, v.z, v.w};
+        const float* wk = wt + c4 * 4 * CO;
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+#pragma unroll
+          for (int co = 0; co < CO; ++co) a[co] = fmaf(vv[e], wk[e * CO + co], a[co]);
       }
     }
   if (ox < W && oy < H) {
     const long plane = (long)H * W;
-    float* o = y + (long)b * 3 * plane + (long)oy * W + ox;
-    o[0] = a0; o[plane] = a1; o[2 * plane] = a2;
+    float* o = y + (long)b * CO * plane + (long)oy * W + ox;
+#pragma unroll
+    for (int co = 0; co < CO; ++co) o[co * plane] = a[co];
   }
 }
 
@@ -295,25 +301,25 @@ extern "C" int femasr_in_conv_pad_weight(const float* w_oihw, float* w_padded, i
   return launch_status("in_conv_weight_pad_kernel");
 }
 
-extern "C" int femasr_out_conv3x3(const float* x, const float* w, const float* bias, float* y, int B, int H, int W,
-                                  int Cin, void* stream) {
-  FEMASR_CHECK_ARG(x && w && bias && y, "out_conv: null pointer");
-  FEMASR_CHECK_ARG(B > 0 && H > 0 && W > 0, "out_conv: empty input");
-  FEMASR_CHECK_ARG(Cin == OC_CIN, "out_conv: Cin must be 64 (channel_query_dict[256])");
-  FEMASR_CHECK_ARG(cdiv(H, OC_TH) <= 65535 && B <= 65535, "out_conv: grid too large");
-  cudaStream_t st = as_stream(stream);
+template <int CO>
+static int out_conv_simt(const float* x, const float* w, const float* bias, float* y, int B, int H, int W, cudaStream_t st) {
   // weights travel through __constant__ memory; refreshed per call (stream-ordered) so several engines can coexist
-  FEMASR_CUDA(cudaMemcpyToSymbolAsync(c_outconv_w, w, sizeof(float) * 9 * OC_CIN * 3, 0, cudaMemcpyDeviceToDevice, st));
-  FEMASR_CUDA(cudaMemcpyToSymbolAsync(c_outconv_b, bias, sizeof(float) * 3, 0, cudaMemcpyDeviceToDevice, st));
+  FEMASR_CUDA(cudaMemcpyToSymbolAsync(c_outconv_w, w, sizeof(float) * 9 * OC_CIN * CO, 0, cudaMemcpyDeviceToDevice, st));
+  FEMASR_CUDA(cudaMemcpyToSymbolAsync(c_outconv_b, bias, sizeof(float) * CO, 0, cudaMemcpyDeviceToDevice, st));
   constexpr int smem = (OC_TH + 2) * (OC_TW + 2) * OC_PS * (int)sizeof(float);
   static PerDeviceFlag attr_set;
   if (!attr_set.cur()) {
-    FEMASR_CUDA(cudaFuncSetAttribute(out_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    FEMASR_CUDA(cudaFuncSetAttribute(out_conv_kernel<CO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_set.cur() = true;
   }
   dim3 grid((unsigned)cdiv(W, OC_TW), (unsigned)cdiv(H, OC_TH), B);
-  out_conv_kernel<<<grid, OC_TH * OC_TW, smem, st>>>(x, y, B, H, W);
+  out_conv_kernel<CO><<<grid, OC_TH * OC_TW, smem, st>>>(x, y, B, H, W);
   return launch_status("out_conv_kernel");
+}
+
+extern "C" int femasr_out_conv3x3(const float* x, const float* w, const float* bias, float* y, int B, int H, int W,
+                                  int Cin, void* stream) {
+  return femasr_out_conv3x3_n(x, w, bias, y, B, H, W, Cin, 3, 0, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -337,19 +343,21 @@ __device__ __forceinline__ void oc_split2(float x, float y, uint32_t& hi, uint32
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(y - hf.y), "f"(x - hf.x));
 }
 
-// w: K-major packed [tap][c][co] fp32 (femasr_pack_weight).  One thread per (kh, kc, nt, reg, lane).
+// w: K-major packed [tap][c][co] fp32 (femasr_pack_weight), CO output channels (3 or 1): the folded N = 3 * CO columns
+// fill one (CO 1) or two (CO 3) 8-wide n-tiles.  One thread per (kh, kc, nt, reg, lane).
+template <int CO>
 __global__ void out_conv_bfrag_kernel(const float* __restrict__ w) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= 3 * 4 * 2 * 2 * 32) return;
   const int lane = idx & 31, reg = (idx >> 5) & 1, nt = (idx >> 6) & 1, kc = (idx >> 7) & 3, kh = idx >> 9;
   const int g = lane >> 2, cq = lane & 3;
-  const int n = nt * 8 + g;                       // column = kw*3 + co
+  const int n = nt * 8 + g;                       // column = kw*CO + co
   float v0 = 0.f, v1 = 0.f;
-  if (n < 9) {
-    const int kw = n / 3, co = n - 3 * kw;
+  if (n < 3 * CO) {
+    const int kw = n / CO, co = n - CO * kw;
     const int ch = 16 * kc + 2 * cq + 8 * reg;    // B fragment: b0 = k 2c,2c+1; b1 = k 2c+8,2c+9
-    v0 = w[(((kh * 3 + kw) * OC_CIN) + ch) * 3 + co] * OM_WSCALE;
-    v1 = w[(((kh * 3 + kw) * OC_CIN) + ch + 1) * 3 + co] * OM_WSCALE;
+    v0 = w[(((kh * 3 + kw) * OC_CIN) + ch) * CO + co] * OM_WSCALE;
+    v1 = w[(((kh * 3 + kw) * OC_CIN) + ch + 1) * CO + co] * OM_WSCALE;
   }
   uint32_t hi, lo;
   oc_split2(v0, v1, hi, lo);
@@ -358,8 +366,10 @@ __global__ void out_conv_bfrag_kernel(const float* __restrict__ w) {
   g_outconv_bfrag[(base + 1 * 2 + reg) * 32 + lane] = lo;
 }
 
+template <int CO>
 __global__ void __launch_bounds__(OM_TH * 32, 2) out_conv_mma_kernel(const float* __restrict__ x, const float* __restrict__ bias,
                                                                      float* __restrict__ y, int B, int H, int W) {
+  constexpr int NC = 3 * CO, NT = (NC + 7) / 8;     // folded columns kw*CO + co, 8-wide n-tiles
   extern __shared__ __align__(16) uint8_t om_smem[];
   uint8_t* plane_hi = om_smem;
   uint8_t* plane_lo = om_smem + OM_PLANE;
@@ -394,21 +404,21 @@ __global__ void __launch_bounds__(OM_TH * 32, 2) out_conv_mma_kernel(const float
   }
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, cq = lane & 3;
-  float acc[2][2][4];
+  float acc[2][NT][4];
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-    for (int nt = 0; nt < 2; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.f;
+    for (int nt = 0; nt < NT; ++nt) acc[mt][nt][0] = acc[mt][nt][1] = acc[mt][nt][2] = acc[mt][nt][3] = 0.f;
   // ldmatrix row address: lane -> pixel (lane & 7) + 8 * ((lane >> 3) & 1) of the m-tile, channel block 8 * (lane >> 4)
   const int lpx = (lane & 7) + 8 * ((lane >> 3) & 1), lch = 8 * (lane >> 4);
   const uint32_t hi_base = (uint32_t)__cvta_generic_to_shared(plane_hi), lo_base = (uint32_t)__cvta_generic_to_shared(plane_lo);
 #pragma unroll 1
   for (int kh = 0; kh < 3; ++kh) {
-    uint32_t bh[4][2][2], bl[4][2][2];            // [kc][nt][reg]
+    uint32_t bh[4][NT][2], bl[4][NT][2];          // [kc][nt][reg]
 #pragma unroll
     for (int kc = 0; kc < 4; ++kc)
 #pragma unroll
-      for (int nt = 0; nt < 2; ++nt)
+      for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           const int base = (((kh * 4 + kc) * 2 + nt) * 2) * 2;
@@ -427,7 +437,7 @@ __global__ void __launch_bounds__(OM_TH * 32, 2) out_conv_mma_kernel(const float
         asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
                      : "=r"(al[0]), "=r"(al[1]), "=r"(al[2]), "=r"(al[3]) : "r"(lo_base + off));
 #pragma unroll
-        for (int nt = 0; nt < 2; ++nt) {
+        for (int nt = 0; nt < NT; ++nt) {
           float(&d)[4] = acc[mt][nt];
           asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
                        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
@@ -441,43 +451,60 @@ __global__ void __launch_bounds__(OM_TH * 32, 2) out_conv_mma_kernel(const float
         }
       }
   }
-  // shift-add over the three horizontal taps through this warp's scratch Q[32 pixels][9]
+  // shift-add over the three horizontal taps through this warp's scratch Q[32 pixels][NC]
   float* qs = qs_all + warp * OM_PX * 9;
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt) {
     const int p0 = mt * 16 + g, p1 = p0 + 8;
-    qs[p0 * 9 + 2 * cq] = acc[mt][0][0]; qs[p0 * 9 + 2 * cq + 1] = acc[mt][0][1];
-    qs[p1 * 9 + 2 * cq] = acc[mt][0][2]; qs[p1 * 9 + 2 * cq + 1] = acc[mt][0][3];
-    if (cq == 0) { qs[p0 * 9 + 8] = acc[mt][1][0]; qs[p1 * 9 + 8] = acc[mt][1][2]; }
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = nt * 8 + 2 * cq + e;
+        if (col < NC) { qs[p0 * NC + col] = acc[mt][nt][e]; qs[p1 * NC + col] = acc[mt][nt][2 + e]; }
+      }
   }
   __syncwarp();
   const int oy = blockIdx.y * OM_TH + warp, ox = blockIdx.x * OM_TW + lane;
   if (lane < OM_TW && oy < H && ox < W) {
     const long plane = (long)H * W;
-    float* o = y + (long)b * 3 * plane + (long)oy * W + ox;
+    float* o = y + (long)b * CO * plane + (long)oy * W + ox;
     const float inv = 1.0f / OM_WSCALE;
 #pragma unroll
-    for (int co = 0; co < 3; ++co)
-      o[co * plane] = __ldg(bias + co) + ((qs[lane * 9 + co] + qs[(lane + 1) * 9 + 3 + co]) + qs[(lane + 2) * 9 + 6 + co]) * inv;
+    for (int co = 0; co < CO; ++co)
+      o[co * plane] = __ldg(bias + co) + ((qs[lane * NC + co] + qs[(lane + 1) * NC + CO + co]) + qs[(lane + 2) * NC + 2 * CO + co]) * inv;
   }
+}
+
+template <int CO>
+static int out_conv_mma(const float* x, const float* w, const float* bias, float* y, int B, int H, int W, cudaStream_t st) {
+  out_conv_bfrag_kernel<CO><<<6, 256, 0, st>>>(w);     // stream-ordered refresh of the B fragments (several engines can coexist)
+  static PerDeviceFlag attr_set;
+  if (!attr_set.cur()) {
+    FEMASR_CUDA(cudaFuncSetAttribute(out_conv_mma_kernel<CO>, cudaFuncAttributeMaxDynamicSharedMemorySize, OM_SMEM));
+    attr_set.cur() = true;
+  }
+  dim3 grid((unsigned)cdiv(W, OM_TW), (unsigned)cdiv(H, OM_TH), B);
+  out_conv_mma_kernel<CO><<<grid, OM_TH * 32, OM_SMEM, st>>>(x, bias, y, B, H, W);
+  return launch_status("out_conv_mma_kernel");
 }
 
 extern "C" int femasr_out_conv3x3_mma(const float* x, const float* w, const float* bias, float* y, int B, int H, int W,
                                       int Cin, void* stream) {
-  FEMASR_CHECK_ARG(x && w && bias && y, "out_conv_mma: null pointer");
-  FEMASR_CHECK_ARG(B > 0 && H > 0 && W > 0, "out_conv_mma: empty input");
-  FEMASR_CHECK_ARG(Cin == OC_CIN, "out_conv_mma: Cin must be 64 (channel_query_dict[256])");
-  FEMASR_CHECK_ARG(cdiv(H, OM_TH) <= 65535 && B <= 65535, "out_conv_mma: grid too large");
+  return femasr_out_conv3x3_n(x, w, bias, y, B, H, W, Cin, 3, 1, stream);
+}
+
+extern "C" int femasr_out_conv3x3_n(const float* x, const float* w, const float* bias, float* y, int B, int H, int W,
+                                    int Cin, int Cout, int mma, void* stream) {
+  const char* what = mma ? "out_conv_mma" : "out_conv";
+  FEMASR_CHECK_ARG(x && w && bias && y, std::string(what) + ": null pointer");
+  FEMASR_CHECK_ARG(B > 0 && H > 0 && W > 0, std::string(what) + ": empty input");
+  FEMASR_CHECK_ARG(Cin == OC_CIN, std::string(what) + ": Cin must be 64 (channel_query_dict[256])");
+  FEMASR_CHECK_ARG(Cout == 3 || Cout == 1, std::string(what) + ": Cout must be 3 or 1");
+  FEMASR_CHECK_ARG(cdiv(H, mma ? OM_TH : OC_TH) <= 65535 && B <= 65535, std::string(what) + ": grid too large");
   cudaStream_t st = as_stream(stream);
-  out_conv_bfrag_kernel<<<6, 256, 0, st>>>(w);     // stream-ordered refresh of the B fragments (several engines can coexist)
-  static PerDeviceFlag attr_set;
-  if (!attr_set.cur()) {
-    FEMASR_CUDA(cudaFuncSetAttribute(out_conv_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, OM_SMEM));
-    attr_set.cur() = true;
-  }
-  dim3 grid((unsigned)cdiv(W, OM_TW), (unsigned)cdiv(H, OM_TH), B);
-  out_conv_mma_kernel<<<grid, OM_TH * 32, OM_SMEM, st>>>(x, bias, y, B, H, W);
-  return launch_status("out_conv_mma_kernel");
+  if (mma) return Cout == 3 ? out_conv_mma<3>(x, w, bias, y, B, H, W, st) : out_conv_mma<1>(x, w, bias, y, B, H, W, st);
+  return Cout == 3 ? out_conv_simt<3>(x, w, bias, y, B, H, W, st) : out_conv_simt<1>(x, w, bias, y, B, H, W, st);
 }
 
 extern "C" int femasr_pack_weight(const float* w, float* out, int Cout, int Cin, int kh, int kw, void* stream) {

@@ -88,6 +88,7 @@ struct ParamInfo {
   size_t numel;
   int Cout, Cin, k;   // conv / linear weight [Cout,Cin,k,k]; codebook [n_e,e_dim] as Cout, Cin, k = 1
   unsigned forms;     // FORM_*
+  std::string sn;     // spectral-norm layer this tensor belongs to (weight_orig / weight_u / weight_v), else empty
 };
 
 // every device buffer of one parameter; nullptr where its ParamInfo lists no such form
@@ -97,7 +98,9 @@ struct DevParam {
   float* relb_mma = nullptr;   // FORM_RELB, fragment order
   float* esq = nullptr;        // FORM_ESQ
   void *tc = nullptr, *tc8 = nullptr, *up = nullptr, *up8 = nullptr, *im2col = nullptr;
-  void release() { for (void* p : {(void*)raw, (void*)packed, (void*)relb_mma, (void*)esq, tc, tc8, up, up8, im2col}) cudaFree(p); }
+  float* sigma = nullptr;      // spectral-norm weight_orig: {u . (W v), |W v|} (femasr_spectral_sigma); the forms above
+  float sn[2] = {0.f, 0.f};    // are packed from weight_orig / sigma.  sn: the same two values on the host
+  void release() { for (void* p : {(void*)raw, (void*)packed, (void*)relb_mma, (void*)esq, tc, tc8, up, up8, im2col, (void*)sigma}) cudaFree(p); }
 };
 
 struct Tap { float* dst; size_t cap; };
@@ -128,6 +131,8 @@ struct femasr_net {
   bool fast_silu = true;                  // approximate-unit SiLU in the operand staging behind the VQ (FEMASR_FAST_SILU=0: exact)
   bool semantic = false;                  // femasr_net_enable_semantic: the VGG19 / conv_semantic tensors are part of the spec
   int sem_slice_kb = 0;                   // K-slice length of the semantic branch's GEMMs (FEMASR_SEM_SLICE_KB; study knob, 0 = one pass)
+  bool disc = false;                      // femasr_disc_create: a UNetDiscriminatorSN (dcfg); cfg holds only gemm_path
+  femasr_disc_config dcfg{};
   std::vector<ProfRec> prof;
   std::string prof_json;
   ~femasr_net() {
@@ -143,14 +148,16 @@ static int chan(int res) {
   return -1;
 }
 
-enum Role { CONV, UP_CONV, IN_CONV, VGG_CONV, VGG_CONV1 };
+// DISC_CONV: a discriminator conv (spectral-norm 3x3 or 4x4 stride 2), never F8
+enum Role { CONV, UP_CONV, IN_CONV, VGG_CONV, VGG_CONV1, DISC_CONV };
 
 static unsigned weight_forms(const femasr_net* n, Role r, int ci, int co, int k) {
   const bool tc = n->cfg.gemm_path == 1;
   if (r == VGG_CONV1 || (r == IN_CONV && tc)) return FORM_KMAJOR | FORM_IM2COL;   // K = 27 / 48 zero-padded to 64
-  if (!tc || (k != 1 && k != 3) || ci % 64 || co % 64) return FORM_KMAJOR;
+  if (!tc || (k != 1 && k != 3 && k != 4) || ci % 64 || co % 64) return FORM_KMAJOR;
   unsigned f = FORM_KMAJOR | FORM_TC;
-  if (n->f8_cross && k == 3 && r != VGG_CONV) f |= FORM_TC8;      // may run behind the VQ; the VGG convs never use F8
+  if (n->f8_cross && k == 3 && r != VGG_CONV && r != DISC_CONV) f |= FORM_TC8;   // may run behind the VQ; the VGG and
+                                                                                  // discriminator convs never use F8
   if (r == UP_CONV) f |= FORM_UP | (n->f8_cross ? FORM_UP8 : 0);
   return f;
 }
@@ -235,6 +242,27 @@ static void add_semantic(femasr_net* n) {
   }
 }
 
+// UNetDiscriminatorSN (discriminator_arch.py): conv0 and conv9 plain convs with bias; conv1 ... conv8 spectral_norm convs
+// without bias, whose state_dict entries are weight_orig [Cout,Cin,k,k], weight_u [Cout] and weight_v [Cin*k*k]
+static void add_sn_conv(femasr_net* n, const std::string& p, int ci, int co, int k) {
+  n->spec[p + ".weight_orig"] = ParamInfo{(size_t)co * ci * k * k, co, ci, k, weight_forms(n, DISC_CONV, ci, co, k), p};
+  n->spec[p + ".weight_u"] = ParamInfo{(size_t)co, 0, 0, 0, 0, p};
+  n->spec[p + ".weight_v"] = ParamInfo{(size_t)ci * k * k, 0, 0, 0, 0, p};
+}
+static void build_disc_spec(femasr_net* n) {
+  const int F = n->dcfg.num_feat;
+  add_conv(n, "conv0", n->dcfg.num_in_ch, F, 3, VGG_CONV1);     // im2col GEMM, K = 27 -> 64
+  add_sn_conv(n, "conv1", F, 2 * F, 4);
+  add_sn_conv(n, "conv2", 2 * F, 4 * F, 4);
+  add_sn_conv(n, "conv3", 4 * F, 8 * F, 4);
+  add_sn_conv(n, "conv4", 8 * F, 4 * F, 3);
+  add_sn_conv(n, "conv5", 4 * F, 2 * F, 3);
+  add_sn_conv(n, "conv6", 2 * F, F, 3);
+  add_sn_conv(n, "conv7", F, F, 3);
+  add_sn_conv(n, "conv8", F, F, 3);
+  add_conv(n, "conv9", F, 1, 3);                                 // femasr_out_conv3x3_n, Cout 1
+}
+
 // ---------------------------------------------------------------------------------------------
 // One conv / linear layer of the graph.  H, W: the conv-input size (low-res when upsample).  The operand is fp32 x, or
 // split-fp16 planes a_hi/a_lo a producer already wrote (tensor-core GEMM only); the result is fp32 y, or split planes
@@ -256,7 +284,9 @@ struct ConvDesc {
   bool bias = true;
   bool im2col = false;                             // the weight's FORM_IM2COL: a 1x1 GEMM over 64-wide im2col rows
   bool semantic = false;                           // a GEMM of the semantic branch (its own numerics)
+  bool sn = false;                                 // a spectral-norm layer: the weight's forms live on w.weight_orig
   int macs = 0;                                    // algorithmic MACs per output element if not Cin*k*k (im2col GEMMs)
+  std::string wname() const { return w + (sn ? ".weight_orig" : ".weight"); }
 };
 
 static ConvDesc geom(const std::string& w, int B, int H, int W, int Cin, int Cout, int k) {
@@ -267,7 +297,7 @@ static ConvDesc geom(const std::string& w, int B, int H, int W, int Cin, int Cou
 
 static double conv_flops(const ConvDesc& d) {   // algorithmic (reference) count
   const int u = d.upsample ? 2 : 1;
-  const int Ho = d.stride == 2 ? (d.H - 1) / 2 + 1 : d.H * u, Wo = d.stride == 2 ? (d.W - 1) / 2 + 1 : d.W * u;
+  const int Ho = d.stride == 2 ? (d.H + 2 - d.k) / 2 + 1 : d.H * u, Wo = d.stride == 2 ? (d.W + 2 - d.k) / 2 + 1 : d.W * u;
   return 2.0 * d.B * Ho * (double)Wo * d.Cout * (d.macs ? d.macs : d.Cin * d.k * d.k);
 }
 
@@ -358,7 +388,7 @@ struct Ctx {
 
   // the wgmma implicit GEMM wherever the spec gave the weight its tensor-core form (gemm_path 1), else the SIMT one
   bool use_tc(const ConvDesc& d) const {
-    return net->cfg.gemm_path == 1 && (d.im2col || has(d.w + ".weight", d.upsample ? FORM_UP : FORM_TC));
+    return net->cfg.gemm_path == 1 && (d.im2col || has(d.wname(), d.upsample ? FORM_UP : FORM_TC));
   }
 
   // The numerics policy.  In front of the VQ (index-critical): every tc_slice_kb k-blocks the tensor core's truncating
@@ -374,16 +404,16 @@ struct Ctx {
       const int nkb = (d.upsample ? 4 : d.k * d.k) * (d.Cin / 64);
       if (net->tc_precise && nkb > net->tc_slice_kb) m.slice_kb = net->tc_slice_kb;
     } else {
-      m.f8 = !d.a_hi && d.k == 3 && d.pro != FEMASR_PRO_LN && has(d.w + ".weight", d.upsample ? FORM_UP8 : FORM_TC8);
+      m.f8 = !d.a_hi && d.k == 3 && d.pro != FEMASR_PRO_LN && has(d.wname(), d.upsample ? FORM_UP8 : FORM_TC8);
       if (d.pro == FEMASR_PRO_GN_SILU && net->fast_silu) m.prologue = FEMASR_PRO_GN_SILU_FAST;
     }
     return m;
   }
 
   const void* weight(const ConvDesc& d, bool tc, bool f8) {
-    const DevParam& p = D(d.w + ".weight");
+    const DevParam& p = D(d.wname());
     const void* w = d.im2col ? p.im2col : !tc ? p.packed : d.upsample ? (f8 ? p.up8 : p.up) : (f8 ? p.tc8 : p.tc);
-    if (!dry() && !w) check(fail(FEMASR_ERR_STATE, "parameter not packed: " + d.w + ".weight"));
+    if (!dry() && !w) check(fail(FEMASR_ERR_STATE, "parameter not packed: " + d.wname()));
     return w;
   }
 
@@ -852,6 +882,102 @@ struct Ctx {
     decode_loop(none, zq, y_nchw, nullptr, nullptr, nullptr, B, h, w);
     ar.release(zq);
   }
+
+  // UNetDiscriminatorSN.forward (discriminator_arch.py), x [B,3,H,W] -> y [B,1,H,W], H and W multiples of 8.  Every conv
+  // is lrelu(conv + bias) [+ skip] in its epilogue (the skip add comes after the activation, like the reference); on
+  // gemm_path 1 they are the K-sliced 3-product split-fp16 GEMM of the precise region (no F8), the bilinear x2 is fused
+  // into the next conv's operand staging, and conv6 -> conv7 -> conv8 hand their outputs on as split planes.
+  void disc(const float* x_nchw, float* y_nchw, int B, int H, int W) {
+    const bool tc = net->cfg.gemm_path == 1, skip = net->dcfg.skip_connection != 0;
+    const int F = net->dcfg.num_feat;
+    precise_region = true;
+    const int hs[4] = {H, H / 2, H / 4, H / 8}, ws[4] = {W, W / 2, W / 4, W / 8};
+    float* xs[4] = {nullptr, nullptr, nullptr, nullptr};   // x0 .. x3, fp32 NHWC; x0 .. x2 live until their skip add
+    auto sn_conv = [&](int i, int h, int w, int ci, int co, int k) {
+      ConvDesc g = geom("conv" + std::to_string(i), B, h, w, ci, co, k);
+      g.name = "disc_conv"; g.sn = true; g.bias = false; g.act = FEMASR_ACT_LRELU;
+      return g;
+    };
+    {  // conv0: 3x3 pad 1, 3 -> F, as a 1x1 GEMM over femasr_vgg_im2col's unnormalised K = 27 (-> 64) rows
+      const size_t rows = (size_t)B * H * W;
+      xs[0] = ar.alloc(rows * F);
+      float *ahi = nullptr, *alo = nullptr, *af = nullptr;
+      if (tc) { ahi = ar.alloc(rows * 32); alo = ar.alloc(rows * 32); } else { af = ar.alloc(rows * 64); }
+      run("disc_im2col", 0.0, [&] { return femasr_vgg_im2col(x_nchw, nullptr, nullptr, ahi, alo, af, B, H, W, st); });
+      ConvDesc g = geom("conv0", B, H, W, 64, F, 1);
+      g.name = "disc_conv"; g.im2col = true; g.macs = 27; g.act = FEMASR_ACT_LRELU;
+      g.x = af; g.a_hi = ahi; g.a_lo = alo; g.y = xs[0];
+      conv(g);
+      if (tc) { ar.release(alo); ar.release(ahi); } else { ar.release(af); }
+    }
+    for (int i = 1; i <= 3; ++i) {   // conv1 .. conv3: 4x4 stride 2 pad 1
+      xs[i] = ar.alloc((size_t)B * hs[i] * ws[i] * (F << i));
+      ConvDesc g = sn_conv(i, hs[i - 1], ws[i - 1], F << (i - 1), F << i, 4);
+      g.stride = 2; g.x = xs[i - 1]; g.y = xs[i];
+      conv(g);
+    }
+    // conv4 .. conv6: 3x3 on bilinear_x2 of the previous output, then + x2 / x1 / x0
+    float* cur = xs[3];
+    void *p_hi = nullptr, *p_lo = nullptr;                 // conv6's output as split planes (tensor-core path)
+    for (int lv = 2; lv >= 0; --lv) {
+      const int ci = F << (lv + 1), co = F << lv, h = hs[lv], w = ws[lv], hl = hs[lv + 1], wl = ws[lv + 1];
+      const size_t n_in = (size_t)B * h * w * ci, n_out = (size_t)B * h * w * co;
+      ConvDesc g = sn_conv(6 - lv, h, w, ci, co, 3);
+      g.res1 = skip ? xs[lv] : nullptr;
+      float *uhi = nullptr, *ulo = nullptr, *uf = nullptr;
+      const float* src = cur;
+      if (tc) {
+        uhi = ar.alloc((n_in + 1) / 2); ulo = ar.alloc((n_in + 1) / 2);
+        run("disc_up", 0.0, [&] {
+          return femasr_tc_prepare(src, uhi, ulo, FEMASR_PRO_BILINEAR2, nullptr, nullptr, nullptr, nullptr, B, hl, wl, ci, 0, 0.f, st);
+        });
+        g.a_hi = uhi; g.a_lo = ulo;
+      } else {
+        uf = ar.alloc(n_in);
+        run("disc_up", 0.0, [&] { return femasr_bilinear_up2(src, uf, B, hl, wl, ci, st); });
+        g.x = uf;
+      }
+      ar.release(cur);
+      cur = nullptr;
+      if (lv == 0 && tc) {
+        p_hi = ar.alloc((n_out + 1) / 2); p_lo = ar.alloc((n_out + 1) / 2);
+        g.o_hi = p_hi; g.o_lo = p_lo;
+      } else {
+        cur = ar.alloc(n_out);
+        g.y = cur;
+      }
+      conv(g);
+      if (tc) { ar.release(ulo); ar.release(uhi); } else { ar.release(uf); }
+      ar.release(xs[lv]);
+    }
+    // conv7, conv8 (3x3 F -> F), then conv9 (3x3 F -> 1, bias) on the out_conv kernels
+    const size_t nf = (size_t)B * H * W * F;
+    ConvDesc g7 = sn_conv(7, H, W, F, F, 3), g8 = sn_conv(8, H, W, F, F, 3);
+    float* x8 = ar.alloc(nf);
+    if (tc) {
+      void* q_hi = ar.alloc((nf + 1) / 2);
+      void* q_lo = ar.alloc((nf + 1) / 2);
+      g7.a_hi = p_hi; g7.a_lo = p_lo; g7.o_hi = q_hi; g7.o_lo = q_lo;
+      conv(g7);
+      ar.release(p_lo); ar.release(p_hi);
+      g8.a_hi = q_hi; g8.a_lo = q_lo; g8.y = x8;
+      conv(g8);
+      ar.release(q_lo); ar.release(q_hi);
+    } else {
+      float* x7 = ar.alloc(nf);
+      g7.x = cur; g7.y = x7;
+      conv(g7);
+      ar.release(cur);
+      g8.x = x7; g8.y = x8;
+      conv(g8);
+      ar.release(x7);
+    }
+    const float *w9 = P("conv9.weight"), *b9 = P("conv9.bias");
+    run("disc_head", 2.0 * 9 * F * (double)B * H * W,
+        [&] { return femasr_out_conv3x3_n(x8, w9, b9, y_nchw, B, H, W, F, 1, tc ? 1 : 0, st); });
+    ar.release(x8);
+    precise_region = false;
+  }
 };
 
 static int check_geometry(femasr_net* net, int B, int H, int W) {
@@ -908,6 +1034,80 @@ static int ensure(T** p, size_t bytes) {
   return FEMASR_OK;
 }
 
+// Packs every device form pi lists into d, from the fp32 tensor src in the reference layout (d.raw, or for a
+// spectral-norm layer weight_orig / sigma).
+static int pack_forms(femasr_net* net, DevParam& d, const ParamInfo& pi, const float* src, cudaStream_t st) {
+  int s = FEMASR_OK;
+  const unsigned f = pi.forms;
+  const int co = pi.Cout, ci = pi.Cin, k = pi.k;
+  const size_t tcb = femasr_tc_weight_bytes(co, ci, k, k), upb = femasr_tc_weight_bytes(4 * co, ci, 2, 2);
+  if ((f & FORM_KMAJOR) && ((s = ensure(&d.packed, pi.numel * sizeof(float))) || (s = femasr_pack_weight(src, d.packed, co, ci, k, k, st))))
+    return s;
+  if (f & FORM_IM2COL) {
+    // the im2col GEMM's weight: the [Cout][64] zero-padded matrix (K = 48 for in_conv, 27 for VGG conv1_1 and the
+    // discriminator's conv0), packed for this net's GEMM path
+    const bool tc = net->cfg.gemm_path == 1;
+    float* tmp = nullptr;
+    FEMASR_CUDA(cudaMallocAsync(&tmp, (size_t)co * 64 * sizeof(float), st));
+    s = k == 4 ? femasr_in_conv_pad_weight(src, tmp, co, st) : femasr_vgg_pad_weight(src, tmp, co, st);
+    if (!s) s = ensure(&d.im2col, tc ? femasr_tc_weight_bytes(co, 64, 1, 1) : (size_t)co * 64 * sizeof(float));
+    if (!s) s = tc ? femasr_tc_pack_weight(tmp, d.im2col, co, 64, 1, 1, st)
+                   : femasr_pack_weight(tmp, static_cast<float*>(d.im2col), co, 64, 1, 1, st);
+    cudaFreeAsync(tmp, st);
+    if (s) return s;
+  }
+  if ((f & FORM_TC) && ((s = ensure(&d.tc, tcb)) || (s = femasr_tc_pack_weight(src, d.tc, co, ci, k, k, st)))) return s;
+  if ((f & FORM_TC8) && ((s = ensure(&d.tc8, tcb)) || (s = femasr_tc_pack_weight_f8(src, d.tc8, co, ci, k, k, st)))) return s;
+  if ((f & FORM_UP) && ((s = ensure(&d.up, upb)) || (s = femasr_tc_pack_weight_up2(src, d.up, co, ci, st)))) return s;
+  if ((f & FORM_UP8) && ((s = ensure(&d.up8, upb)) || (s = femasr_tc_pack_weight_up2_f8(src, d.up8, co, ci, st)))) return s;
+  if ((f & FORM_RELB) &&
+      ((s = ensure(&d.packed, 8 * 64 * 64 * sizeof(float))) || (s = ensure(&d.relb_mma, 8 * 64 * 64 * sizeof(float))) ||
+       (s = femasr_expand_rel_bias_mma(src, d.relb_mma, 8, st)) || (s = femasr_expand_rel_bias(src, d.packed, 8, st))))
+    return s;
+  if ((f & FORM_ESQ) && ((s = ensure(&d.esq, co * sizeof(float))) || (s = femasr_row_sumsq(src, d.esq, co, ci, st)))) return s;
+  return FEMASR_OK;
+}
+
+// Spectral-norm layer l (eval mode, torch.nn.utils.spectral_norm): once weight_orig, weight_u and weight_v are all set,
+// sigma = u . (W v) and the layer's forms are packed from weight_orig / sigma.  The host copy of {sigma, |W v|} feeds
+// the gemm_path 1 range check of femasr_disc_forward.
+static int sn_pack(femasr_net* net, const std::string& l, cudaStream_t st) {
+  auto w = net->dev.find(l + ".weight_orig"), u = net->dev.find(l + ".weight_u"), v = net->dev.find(l + ".weight_v");
+  if (w == net->dev.end() || u == net->dev.end() || v == net->dev.end()) return FEMASR_OK;
+  const ParamInfo& pi = net->spec.at(l + ".weight_orig");
+  DevParam& d = w->second;
+  int s = ensure(&d.sigma, 2 * sizeof(float));
+  if (s) return s;
+  float* wn = nullptr;
+  FEMASR_CUDA(cudaMallocAsync(&wn, pi.numel * sizeof(float), st));
+  s = femasr_spectral_sigma(d.raw, u->second.raw, v->second.raw, pi.Cout, (int)(pi.numel / pi.Cout), d.sigma, st);
+  if (!s) s = femasr_spectral_normalize(d.raw, d.sigma, wn, pi.numel, st);
+  if (!s) s = pack_forms(net, d, pi, wn, st);
+  cudaFreeAsync(wn, st);
+  if (s) return s;
+  FEMASR_CUDA(cudaMemcpyAsync(d.sn, d.sigma, 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  FEMASR_CUDA(cudaStreamSynchronize(st));
+  return FEMASR_OK;
+}
+
+static int check_disc_geometry(int B, int H, int W) {
+  if (B <= 0 || H <= 0 || W <= 0) return fail(FEMASR_ERR_ARG, "disc: empty input");
+  if (H % 8 || W % 8)
+    return fail(FEMASR_ERR_ARG, "disc: H and W must be multiples of 8 (three stride-2 convs, then x2 upsamples that must "
+                                "meet the skip tensors; the reference raises at the skip add)");
+  return FEMASR_OK;
+}
+
+// Study knobs read from the environment at create time (generator and discriminator alike)
+static void read_knobs(femasr_net* n) {
+  if (const char* ev = getenv("FEMASR_TC_PRECISE")) n->tc_precise = atoi(ev) != 0;
+  if (const char* ev = getenv("FEMASR_FAST_SILU")) n->fast_silu = atoi(ev) != 0;
+  if (const char* ev = getenv("FEMASR_VQ_FUSED")) n->vq_fused = atoi(ev) != 0;
+  if (const char* ev = getenv("FEMASR_F8_CROSS")) n->f8_cross = atoi(ev) != 0;
+  if (const char* ev = getenv("FEMASR_TC_SLICE_KB")) n->tc_slice_kb = std::max(1, atoi(ev));
+  if (const char* ev = getenv("FEMASR_SEM_SLICE_KB")) n->sem_slice_kb = std::max(0, atoi(ev));
+}
+
 }  // namespace femasr
 
 extern "C" const char* femasr_last_error(void) { return g_err.c_str(); }
@@ -951,12 +1151,7 @@ extern "C" int femasr_net_create(const femasr_net_config* cfg, femasr_net** out)
   }
   n->depth = cfg->scale_factor == 4 ? 1 : (cfg->scale_factor == 2 ? 2 : 3);
   n->hq = cfg->scale_factor == 1;
-  if (const char* ev = getenv("FEMASR_TC_PRECISE")) n->tc_precise = atoi(ev) != 0;
-  if (const char* ev = getenv("FEMASR_FAST_SILU")) n->fast_silu = atoi(ev) != 0;
-  if (const char* ev = getenv("FEMASR_VQ_FUSED")) n->vq_fused = atoi(ev) != 0;
-  if (const char* ev = getenv("FEMASR_F8_CROSS")) n->f8_cross = atoi(ev) != 0;
-  if (const char* ev = getenv("FEMASR_TC_SLICE_KB")) n->tc_slice_kb = std::max(1, atoi(ev));
-  if (const char* ev = getenv("FEMASR_SEM_SLICE_KB")) n->sem_slice_kb = std::max(0, atoi(ev));
+  read_knobs(n);
   build_spec(n);
   *out = n;
   return FEMASR_OK;
@@ -966,6 +1161,7 @@ extern "C" void femasr_net_destroy(femasr_net* net) { delete net; }
 
 extern "C" int femasr_net_enable_semantic(femasr_net* net) {
   FEMASR_CHECK_ARG(net, "enable_semantic: null");
+  FEMASR_CHECK_ARG(!net->disc, "enable_semantic: a discriminator handle");
   if (net->semantic) return FEMASR_OK;
   if (!net->dev.empty()) return fail(FEMASR_ERR_STATE, "enable_semantic: call it before the first set_param");
   add_semantic(net);
@@ -987,34 +1183,8 @@ extern "C" int femasr_net_set_param(femasr_net* net, const char* name, const flo
   if (s) return s;
   FEMASR_CUDA(cudaMemcpyAsync(d.raw, data, numel * sizeof(float), on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
   if (!on_device) FEMASR_CUDA(cudaStreamSynchronize(st));   // the host buffer may be pageable / freed by the caller
-  const unsigned f = pi.forms;
-  const int co = pi.Cout, ci = pi.Cin, k = pi.k;
-  const size_t tcb = femasr_tc_weight_bytes(co, ci, k, k), upb = femasr_tc_weight_bytes(4 * co, ci, 2, 2);
-  if ((f & FORM_KMAJOR) && ((s = ensure(&d.packed, numel * sizeof(float))) || (s = femasr_pack_weight(d.raw, d.packed, co, ci, k, k, st))))
-    return s;
-  if (f & FORM_IM2COL) {
-    // the im2col GEMM's weight: the [Cout][64] zero-padded matrix (K = 48 for in_conv, 27 for VGG conv1_1), packed
-    // for this net's GEMM path
-    const bool tc = net->cfg.gemm_path == 1;
-    float* tmp = nullptr;
-    FEMASR_CUDA(cudaMallocAsync(&tmp, (size_t)co * 64 * sizeof(float), st));
-    s = k == 4 ? femasr_in_conv_pad_weight(d.raw, tmp, co, st) : femasr_vgg_pad_weight(d.raw, tmp, co, st);
-    if (!s) s = ensure(&d.im2col, tc ? femasr_tc_weight_bytes(co, 64, 1, 1) : (size_t)co * 64 * sizeof(float));
-    if (!s) s = tc ? femasr_tc_pack_weight(tmp, d.im2col, co, 64, 1, 1, st)
-                   : femasr_pack_weight(tmp, static_cast<float*>(d.im2col), co, 64, 1, 1, st);
-    cudaFreeAsync(tmp, st);
-    if (s) return s;
-  }
-  if ((f & FORM_TC) && ((s = ensure(&d.tc, tcb)) || (s = femasr_tc_pack_weight(d.raw, d.tc, co, ci, k, k, st)))) return s;
-  if ((f & FORM_TC8) && ((s = ensure(&d.tc8, tcb)) || (s = femasr_tc_pack_weight_f8(d.raw, d.tc8, co, ci, k, k, st)))) return s;
-  if ((f & FORM_UP) && ((s = ensure(&d.up, upb)) || (s = femasr_tc_pack_weight_up2(d.raw, d.up, co, ci, st)))) return s;
-  if ((f & FORM_UP8) && ((s = ensure(&d.up8, upb)) || (s = femasr_tc_pack_weight_up2_f8(d.raw, d.up8, co, ci, st)))) return s;
-  if ((f & FORM_RELB) &&
-      ((s = ensure(&d.packed, 8 * 64 * 64 * sizeof(float))) || (s = ensure(&d.relb_mma, 8 * 64 * 64 * sizeof(float))) ||
-       (s = femasr_expand_rel_bias_mma(d.raw, d.relb_mma, 8, st)) || (s = femasr_expand_rel_bias(d.raw, d.packed, 8, st))))
-    return s;
-  if ((f & FORM_ESQ) && ((s = ensure(&d.esq, co * sizeof(float))) || (s = femasr_row_sumsq(d.raw, d.esq, co, ci, st)))) return s;
-  return FEMASR_OK;
+  if (!pi.sn.empty()) return sn_pack(net, pi.sn, st);
+  return pack_forms(net, d, pi, d.raw, st);
 }
 
 extern "C" int femasr_net_params_complete(femasr_net* net) {
@@ -1026,11 +1196,13 @@ extern "C" int femasr_net_params_complete(femasr_net* net) {
 
 extern "C" int femasr_net_workspace_bytes(femasr_net* net, int B, int H, int W, size_t* bytes) {
   FEMASR_CHECK_ARG(net && bytes, "workspace_bytes: null pointer");
+  FEMASR_CHECK_ARG(!net->disc, "workspace_bytes: a discriminator handle (use femasr_disc_workspace_bytes)");
   return workspace_impl(net, B, H, W, false, bytes);
 }
 
 extern "C" int femasr_net_workspace_bytes_sem(femasr_net* net, int B, int H, int W, int with_sem, size_t* bytes) {
   FEMASR_CHECK_ARG(net && bytes, "workspace_bytes_sem: null pointer");
+  FEMASR_CHECK_ARG(!net->disc, "workspace_bytes_sem: a discriminator handle (use femasr_disc_workspace_bytes)");
   return workspace_impl(net, B, H, W, with_sem != 0, bytes);
 }
 
@@ -1049,6 +1221,7 @@ extern "C" int femasr_net_forward_sem(femasr_net* net, const float* x, float* y,
                                       const int64_t* gt_indices, float* sem_loss, int B, int H, int W, void* workspace,
                                       size_t workspace_bytes, void* stream) {
   FEMASR_CHECK_ARG(net && x && y && workspace, "forward: null pointer");
+  FEMASR_CHECK_ARG(!net->disc, "forward: a discriminator handle (use femasr_disc_forward)");
   int s = check_geometry(net, B, H, W);
   if (s) return s;
   s = femasr_net_params_complete(net);
@@ -1065,6 +1238,7 @@ extern "C" int femasr_net_forward_sem(femasr_net* net, const float* x, float* y,
 
 extern "C" int femasr_net_decode_workspace_bytes(femasr_net* net, int B, int h, int w, size_t* bytes) {
   FEMASR_CHECK_ARG(net && bytes && B > 0 && h > 0 && w > 0, "decode_workspace_bytes: bad argument");
+  FEMASR_CHECK_ARG(!net->disc, "decode_workspace_bytes: a discriminator handle");
   Ctx c(net, nullptr, 0, nullptr);
   c.decode_indices(nullptr, nullptr, B, h, w);
   *bytes = c.bytes_needed();
@@ -1074,6 +1248,7 @@ extern "C" int femasr_net_decode_workspace_bytes(femasr_net* net, int B, int h, 
 extern "C" int femasr_net_decode_indices(femasr_net* net, const int64_t* indices, float* y, int B, int h, int w,
                                          void* workspace, size_t workspace_bytes, void* stream) {
   FEMASR_CHECK_ARG(net && indices && y && workspace && B > 0 && h > 0 && w > 0, "decode_indices: bad argument");
+  FEMASR_CHECK_ARG(!net->disc, "decode_indices: a discriminator handle");
   int s = femasr_net_params_complete(net);
   if (s) return s;
   size_t need = 0;
@@ -1087,6 +1262,7 @@ extern "C" int femasr_net_decode_indices(femasr_net* net, const int64_t* indices
 
 extern "C" int femasr_net_set_tap(femasr_net* net, const char* stage, float* dst, size_t capacity) {
   FEMASR_CHECK_ARG(net && stage, "set_tap: null pointer");
+  FEMASR_CHECK_ARG(!net->disc, "set_tap: a discriminator handle");
   static const char* names[] = {"in_conv", "down", "swin", "up1", "up2", "z", "zq", "after_quant", "dec0", "dec1", "dec2", "z1", "z2",
                                 "vgg", "semantic"};
   bool known = false;
@@ -1136,11 +1312,79 @@ extern "C" const char* femasr_net_profile_json(femasr_net* net) {
 // The sum of the algorithmic FLOPs the launches of one plain forward report (no taps, no gt_indices, no semantic loss),
 // counted by a sizing run; 0 for a geometry forward rejects.
 extern "C" double femasr_net_flops(femasr_net* net, int B, int H, int W) {
-  if (!net || check_geometry(net, B, H, W)) return 0.0;
+  if (!net || net->disc || check_geometry(net, B, H, W)) return 0.0;
   std::map<std::string, Tap> taps;
   taps.swap(net->taps);          // a registered in_conv tap adds the fp32 in_conv to the tensor-core plan
   Ctx c(net, nullptr, 0, nullptr);
   c.forward(nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W);
   taps.swap(net->taps);
+  return c.flops;
+}
+
+// ------------------------------------------------------------------------------------------------ UNetDiscriminatorSN
+extern "C" int femasr_disc_create(const femasr_disc_config* cfg, femasr_net** out) {
+  FEMASR_CHECK_ARG(cfg && out, "disc_create: null pointer");
+  FEMASR_CHECK_ARG(cfg->num_in_ch == 3, "disc_create: num_in_ch must be 3");
+  FEMASR_CHECK_ARG(cfg->num_feat == 64, "disc_create: num_feat must be 64 (conv9 runs on the Cin = 64 head kernels)");
+  FEMASR_CHECK_ARG(cfg->skip_connection == 0 || cfg->skip_connection == 1, "disc_create: skip_connection must be 0 or 1");
+  FEMASR_CHECK_ARG(cfg->gemm_path == 0 || cfg->gemm_path == 1, "disc_create: gemm_path must be 0 or 1");
+  femasr_net* n = new femasr_net();
+  n->cfg = femasr_net_config{};
+  n->cfg.gemm_path = cfg->gemm_path;
+  n->disc = true;
+  n->dcfg = *cfg;
+  read_knobs(n);
+  build_disc_spec(n);
+  *out = n;
+  return FEMASR_OK;
+}
+
+extern "C" int femasr_disc_workspace_bytes(femasr_net* net, int B, int H, int W, size_t* bytes) {
+  FEMASR_CHECK_ARG(net && bytes, "disc_workspace_bytes: null pointer");
+  FEMASR_CHECK_ARG(net->disc, "disc_workspace_bytes: a generator handle (use femasr_net_workspace_bytes)");
+  int s = check_disc_geometry(B, H, W);
+  if (s) return s;
+  Ctx c(net, nullptr, 0, nullptr);
+  c.disc(nullptr, nullptr, B, H, W);
+  *bytes = c.bytes_needed();
+  return c.status;
+}
+
+extern "C" int femasr_disc_forward(femasr_net* net, const float* x, float* y, int B, int H, int W, void* workspace,
+                                   size_t workspace_bytes, void* stream) {
+  FEMASR_CHECK_ARG(net && x && y && workspace, "disc_forward: null pointer");
+  FEMASR_CHECK_ARG(net->disc, "disc_forward: a generator handle (use femasr_net_forward)");
+  int s = check_disc_geometry(B, H, W);
+  if (s) return s;
+  s = femasr_net_params_complete(net);
+  if (s) return s;
+  if (net->cfg.gemm_path == 1) {
+    // u never power-iterated: sigma = u.(W v) is a small fraction of the spectral norm, the normalised weights are large
+    // and the activations leave the fp16 operand range (a finite reference result would come back as inf)
+    for (auto& kv : net->spec) {
+      if (kv.second.sn.empty() || kv.first != kv.second.sn + ".weight_orig") continue;
+      const float* sn = net->dev.at(kv.first).sn;
+      if (!(sn[0] >= 0.5f * sn[1]))
+        return fail(FEMASR_ERR_STATE, kv.second.sn + ": u.(W v) = " + std::to_string(sn[0]) + " is below half of |W v| = " +
+                                          std::to_string(sn[1]) + ": weight_u / weight_v were never power-iterated, and " +
+                                          "gemm_path 1's fp16 operands cannot hold the activations; use gemm_path 0 or "
+                                          "iterated u, v (as a trained checkpoint carries)");
+    }
+  }
+  size_t need = 0;
+  s = femasr_disc_workspace_bytes(net, B, H, W, &need);
+  if (s) return s;
+  if (workspace_bytes < need) return fail(FEMASR_ERR_STATE, "disc_forward: workspace too small (need " + std::to_string(need) + " bytes)");
+  Ctx c(net, workspace, workspace_bytes, stream);
+  c.disc(x, y, B, H, W);
+  return c.finish();
+}
+
+// The sum of the algorithmic FLOPs of one femasr_disc_forward's launches, counted by a sizing run; 0 for a rejected
+// geometry or a generator handle.
+extern "C" double femasr_disc_flops(femasr_net* net, int B, int H, int W) {
+  if (!net || !net->disc || check_disc_geometry(B, H, W)) return 0.0;
+  Ctx c(net, nullptr, 0, nullptr);
+  c.disc(nullptr, nullptr, B, H, W);
   return c.flops;
 }

@@ -152,6 +152,7 @@ __global__ void __launch_bounds__(256, 2) igemm_simt_kernel(const IgemmP p) {
       }
       if (p.act == FEMASR_ACT_GELU) { o.x = gelu_erf_f(o.x); o.y = gelu_erf_f(o.y); o.z = gelu_erf_f(o.z); o.w = gelu_erf_f(o.w); }
       else if (p.act == FEMASR_ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+      else if (p.act == FEMASR_ACT_LRELU) { o.x = lrelu02_f(o.x); o.y = lrelu02_f(o.y); o.z = lrelu02_f(o.z); o.w = lrelu02_f(o.w); }
       const long off = m * p.Cout + n;
       if (p.res1) {
         const float4 r = *reinterpret_cast<const float4*>(p.res1 + off);
@@ -184,7 +185,13 @@ int igemm_out_dims(const femasr_igemm_args* a, int* Ho, int* Wo) {
     *Ho = a->Hin; *Wo = a->Win;
     return FEMASR_OK;
   }
-  if (a->ksize != 3) return fail(FEMASR_ERR_ARG, "igemm: ksize must be 1 or 3");
+  if (a->ksize == 4) {      // 4x4 pad 1 stride 2 (UNetDiscriminatorSN's down convs)
+    if (a->stride != 2 || a->upsample) return fail(FEMASR_ERR_ARG, "igemm: 4x4 supports stride 2, no upsample");
+    if (a->Hin < 2 || a->Win < 2) return fail(FEMASR_ERR_ARG, "igemm: a 4x4 stride-2 conv needs Hin, Win >= 2");
+    *Ho = (a->Hin + 2 - 4) / 2 + 1; *Wo = (a->Win + 2 - 4) / 2 + 1;
+    return FEMASR_OK;
+  }
+  if (a->ksize != 3) return fail(FEMASR_ERR_ARG, "igemm: ksize must be 1, 3 or 4");
   const int He = a->upsample ? 2 * a->Hin : a->Hin, We = a->upsample ? 2 * a->Win : a->Win;
   if (a->stride == 1) { *Ho = He; *Wo = We; }
   else if (a->stride == 2) { *Ho = (He + 2 - 3) / 2 + 1; *Wo = (We + 2 - 3) / 2 + 1; }
@@ -208,7 +215,7 @@ extern "C" int femasr_igemm_simt(const femasr_igemm_args* a, void* stream) {
   p.x = a->x; p.w = a->w; p.bias = a->bias; p.res1 = a->res1; p.res2 = a->res2; p.y = a->y;
   p.pro_a = a->pro_a; p.pro_b = a->pro_b; p.gamma = a->gamma; p.beta = a->beta;
   p.B = a->B; p.Hin = a->Hin; p.Win = a->Win; p.Cin = a->Cin; p.Cout = a->Cout;
-  p.ksize = a->ksize; p.stride = a->stride; p.upsample = a->upsample; p.pad = a->ksize == 3 ? 1 : 0;
+  p.ksize = a->ksize; p.stride = a->stride; p.upsample = a->upsample; p.pad = a->ksize == 1 ? 0 : 1;
   p.act = a->act;
   p.M = (long)a->B * p.Ho * p.Wo;
   if (a->Cout % 128 == 0) return launch_bn<128>(p, a->prologue, as_stream(stream));

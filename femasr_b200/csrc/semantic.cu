@@ -10,6 +10,7 @@ namespace femasr {
 
 // conv1_1's operand: per output pixel the 3x3x3 window of (x - mean) / std (vgg_arch.py forward: division, not a
 // multiply by 1/std), k = (kh * 3 + kw) * 3 + ci, zero padded to K = 64.  Thread = (pixel, 8-wide k chunk).
+// mean == NULL: the window of x itself (the discriminator's conv0).
 __global__ void __launch_bounds__(256) vgg_im2col_kernel(const float* __restrict__ x, const float* __restrict__ mean,
                                                          const float* __restrict__ stdv, uint4* __restrict__ hi,
                                                          uint4* __restrict__ lo, float4* __restrict__ f32, int H, int W,
@@ -30,8 +31,10 @@ __global__ void __launch_bounds__(256) vgg_im2col_kernel(const float* __restrict
     if (k < 27) {
       const int tap = k / 3, ci = k - tap * 3;
       const int iy = oy + tap / 3 - 1, ix = ox + tap % 3 - 1;
-      if (iy >= 0 && iy < H && ix >= 0 && ix < W)
-        v[e] = __fdiv_rn(__fsub_rn(__ldg(x + ((b * 3 + ci) * H + iy) * W + ix), __ldg(mean + ci)), __ldg(stdv + ci));
+      if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
+        const float px = __ldg(x + ((b * 3 + ci) * H + iy) * W + ix);
+        v[e] = mean ? __fdiv_rn(__fsub_rn(px, __ldg(mean + ci)), __ldg(stdv + ci)) : px;   // NULL mean/std: raw image
+      }
     }
   }
   if (f32) {
@@ -93,7 +96,8 @@ using namespace femasr;
 
 extern "C" int femasr_vgg_im2col(const float* x, const float* mean, const float* std_, void* a_hi, void* a_lo, float* a_f32,
                                  int B, int H, int W, void* stream) {
-  FEMASR_CHECK_ARG(x && mean && std_ && B > 0 && H > 0 && W > 0, "vgg_im2col: bad argument");
+  FEMASR_CHECK_ARG(x && B > 0 && H > 0 && W > 0, "vgg_im2col: bad argument");
+  FEMASR_CHECK_ARG(!mean == !std_, "vgg_im2col: give both mean and std, or neither (no normalisation)");
   FEMASR_CHECK_ARG(a_f32 ? (!a_hi && !a_lo) : (a_hi && a_lo), "vgg_im2col: give either a_hi/a_lo or a_f32");
   const long total = (long)B * H * W * 8;
   vgg_im2col_kernel<<<(unsigned)cdiv(total, 256), 256, 0, as_stream(stream)>>>(

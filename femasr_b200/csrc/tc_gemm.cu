@@ -1,4 +1,4 @@
-// Hopper (sm_90a) tensor-core implicit GEMM (3x3 convolution, stride 1 or 2, the fused nearest-x2 upsample conv, and
+// Hopper (sm_90a) tensor-core implicit GEMM (3x3 convolution, stride 1 or 2, 4x4 stride 2, the fused nearest-x2 upsample conv, and
 // linear layers) with fp32-grade accuracy from a two-term fp16 operand split:
 //
 //     a = a_hi + a_lo,  w*2^s = w_hi + w_lo          (fp16, 11-bit significands each)
@@ -212,7 +212,9 @@ __device__ __forceinline__ void top4_insert(float (&td)[4], int (&tj)[4], float 
 // inside the k-loop makes ptxas serialise every wgmma of the kernel.
 // VQ: the z . E^T product of the VectorQuantizer with the argmin fused into the epilogue (see the VQ epilogue below);
 // work is ordered M-major so that one CTA sees ALL code tiles of its 128 feature rows back to back.
-template <int BN, bool RES, bool F8, bool VQ = false>
+// EXT: the discriminator's additions, 4x4 taps and the LeakyReLU epilogue.  A template parameter so that the other
+// instantiations keep exactly the instruction stream they had without them (measured: 1.3% slower GEMMs otherwise).
+template <int BN, bool RES, bool F8, bool VQ = false, bool EXT = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                 const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const TcP p) {
@@ -263,7 +265,7 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
   if (warp == TC_CONSUMER_WARPS) {
     // ===================== TMA producer =====================
     if (!elect_one()) return;
-    const int ksz = p.taps == 9 ? 3 : 1;   // (p.up: taps == 4, offsets from the phase)
+    const int ksz = EXT && p.taps == 16 ? 4 : (p.taps == 9 ? 3 : 1);   // (p.up: taps == 4, offsets from the phase)
     int stage = 0; uint32_t phase = 0;
     for (int it = 0, work; (work = work_of(it)) >= 0; ++it) {
       const TileCoord tc = decode(work);
@@ -275,6 +277,7 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
         int dy = 0, dx = 0;
         if (p.up) { dy = (tap >> 1) - 1 + (tc.ph >> 1); dx = (tap & 1) - 1 + (tc.ph & 1); }
         else if (ksz == 3) { dy = tap / 3 - 1; dx = tap - (tap / 3) * 3 - 1; }
+        else if (EXT && ksz == 4) { dy = (tap >> 2) - 1; dx = (tap & 3) - 1; }     // 4x4 pad 1, always stride 2
         const int x = p.stride * tc.tx * p.Wt + dx, y = p.stride * tc.ty * p.Ht + dy;
         mbar_wait(empty_bar(stage), phase ^ 1u);
         const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
@@ -429,6 +432,7 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
         o.y = fmaf(acc[4 * j + 2 * h + 1], inv_scale, bb.y);
         if (p.act == FEMASR_ACT_GELU) { o.x = gelu_erf_fast_f(o.x); o.y = gelu_erf_fast_f(o.y); }
         else if (p.act == FEMASR_ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+        else if (EXT && p.act == FEMASR_ACT_LRELU) { o.x = lrelu02_f(o.x); o.y = lrelu02_f(o.y); }
         if (off[h] >= 0) {
           const long o_off = off[h] + col;
           if (RES) { const float2 r = *reinterpret_cast<const float2*>(p.res1 + o_off); o.x += r.x; o.y += r.y; }
@@ -536,6 +540,17 @@ __global__ void __launch_bounds__(256) tc_prepare_pool_kernel(const float* __res
   if (i >= total8) return;
   float v[8];
   const long o = pool2_max8(x, i, H, W, C, v);
+  split_store8(v, hi + o, lo + o);
+}
+
+// Bilinear x2 (align_corners=False) fused into the staging the same way: interpolated on fp32, then split.
+// x [B,H,W,C] -> [B,2H,2W,C], 8 channels per thread.
+__global__ void __launch_bounds__(256) tc_prepare_bilinear_kernel(const float* __restrict__ x, __half* __restrict__ hi,
+                                                                  __half* __restrict__ lo, int H, int W, int C, long total8) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total8) return;
+  float v[8];
+  const long o = bilinear2_8(x, i, H, W, C, v);
   split_store8(v, hi + o, lo + o);
 }
 
@@ -848,18 +863,18 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
-template <int BN, bool RES, bool F8, bool VQ>
+template <int BN, bool RES, bool F8, bool VQ, bool EXT = false>
 static int launch_tc_v(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
                        const TcP& p, cudaStream_t st) {
   using Cfg = TcCfg<BN>;
   static PerDeviceFlag attr_set;      // per template instantiation AND per device
   if (!attr_set.cur()) {
-    FEMASR_CUDA(cudaFuncSetAttribute(tc_igemm_kernel<BN, RES, F8, VQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    FEMASR_CUDA(cudaFuncSetAttribute(tc_igemm_kernel<BN, RES, F8, VQ, EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set.cur() = true;
   }
   const int items = VQ ? p.num_tiles / p.n_tiles : p.num_tiles;     // VQ: one CTA walks all code tiles of an m-tile
   const int grid = items < sm_count() ? items : sm_count();
-  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ>, dim3(grid), dim3(TC_THREADS), Cfg::SMEM_BYTES, st, ah, al, bh, bl, p));
+  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ, EXT>, dim3(grid), dim3(TC_THREADS), Cfg::SMEM_BYTES, st, ah, al, bh, bl, p));
   return launch_status(VQ ? "tc_igemm_kernel(vq)" : "tc_igemm_kernel");
 }
 
@@ -867,6 +882,8 @@ template <int BN>
 static int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
                      const TcP& p, cudaStream_t st) {
   if (p.f8) return p.res1 ? launch_tc_v<BN, true, true, false>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, true, false>(ah, al, bh, bl, p, st);
+  if (p.taps == 16 || p.act == FEMASR_ACT_LRELU)
+    return p.res1 ? launch_tc_v<BN, true, false, false, true>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false, true>(ah, al, bh, bl, p, st);
   return p.res1 ? launch_tc_v<BN, true, false, false>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false>(ah, al, bh, bl, p, st);
 }
 
@@ -902,7 +919,7 @@ static TilePlan plan_tiles(const femasr_tc_args* a, int H, int W) {
 extern "C" int femasr_tc_gn_partial_rows(const femasr_tc_args* a) {
   if (!a) return 0;
   int H = a->H, W = a->W;
-  if (a->stride == 2) { H = (H - 1) / 2 + 1; W = (W - 1) / 2 + 1; }
+  if (a->stride == 2) { H = (H + 2 - a->ksize) / 2 + 1; W = (W + 2 - a->ksize) / 2 + 1; }
   const TilePlan t = plan_tiles(a, H, W);
   return (a->upsample ? 4 : 1) * t.tiles_x * t.tiles_y * 4;
 }
@@ -1004,6 +1021,12 @@ extern "C" int femasr_tc_prepare(const float* x, void* a_hi, void* a_lo, int mod
     tc_prepare_pool_kernel<<<(unsigned)cdiv(total8, 256), 256, 0, st>>>(x, hi, lo, H, W, C, total8);
     return launch_status("tc_prepare_pool_kernel");
   }
+  if (mode == FEMASR_PRO_BILINEAR2) {
+    FEMASR_CHECK_ARG(!upsample, "tc_prepare: bilinear mode has its own x2 (upsample must be 0)");
+    const long total8 = (long)B * 2 * H * 2 * W * (C / 8);
+    tc_prepare_bilinear_kernel<<<(unsigned)cdiv(total8, 256), 256, 0, st>>>(x, hi, lo, H, W, C, total8);
+    return launch_status("tc_prepare_bilinear_kernel");
+  }
   static const int flat_env = [] { const char* e = getenv("FEMASR_PREP_FLAT"); return e ? atoi(e) : 1; }();
   if (!upsample && flat_env && (long)H * W * (C / 4) < (1l << 30) && B <= 65535 &&
       (mode == FEMASR_PRO_GN_SILU || mode == FEMASR_PRO_GN_SILU_FAST || mode == FEMASR_PRO_NONE)) {
@@ -1084,16 +1107,18 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
   FEMASR_CHECK_ARG(a->y || (a->out_hi && a->out_lo), "tc_igemm: need y or the out_hi/out_lo planes");
   FEMASR_CHECK_ARG(!a->out_hi == !a->out_lo, "tc_igemm: out_hi and out_lo go together");
   FEMASR_CHECK_ARG(a->B > 0 && a->H > 0 && a->W > 0, "tc_igemm: empty input");
-  FEMASR_CHECK_ARG(a->ksize == 1 || a->ksize == 3, "tc_igemm: ksize must be 1 or 3");
+  FEMASR_CHECK_ARG(a->ksize == 1 || a->ksize == 3 || a->ksize == 4, "tc_igemm: ksize must be 1, 3 or 4");
   FEMASR_CHECK_ARG(!a->upsample || a->ksize == 3, "tc_igemm: upsample fusion needs ksize 3 (and an up2 weight blob)");
   FEMASR_CHECK_ARG(a->Cin % 64 == 0 && a->Cout % 64 == 0, "tc_igemm: Cin and Cout must be multiples of 64");
   int B = a->B, H = a->H, W = a->W;
   const int stride = a->stride == 2 ? 2 : 1;
   FEMASR_CHECK_ARG(a->stride >= 0 && a->stride <= 2, "tc_igemm: stride must be 1 or 2");
-  FEMASR_CHECK_ARG(stride == 1 || (a->ksize == 3 && !a->upsample), "tc_igemm: stride 2 needs a plain 3x3 conv");
+  FEMASR_CHECK_ARG(stride == 1 || (a->ksize != 1 && !a->upsample), "tc_igemm: stride 2 needs a plain 3x3 or 4x4 conv");
+  FEMASR_CHECK_ARG(a->ksize != 4 || stride == 2, "tc_igemm: ksize 4 needs stride 2");
+  FEMASR_CHECK_ARG(a->ksize != 4 || (H >= 2 && W >= 2), "tc_igemm: a 4x4 stride-2 conv needs H, W >= 2");
   if (a->ksize == 1) { W = B * H * W; H = 1; B = 1; }     // pointwise: one long row of tokens
   const int Hin = H, Win = W;                             // activation-plane dims
-  if (stride == 2) { H = (H - 1) / 2 + 1; W = (W - 1) / 2 + 1; }   // tiles run over the output grid
+  if (stride == 2) { H = (H + 2 - a->ksize) / 2 + 1; W = (W + 2 - a->ksize) / 2 + 1; }   // tiles run over the output grid
   FEMASR_CHECK_ARG((long)W < (1l << 31), "tc_igemm: too many rows");
   const int taps = a->upsample ? 4 : a->ksize * a->ksize;
   const int phases = a->upsample ? 4 : 1;
@@ -1114,6 +1139,7 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
   p.up = a->upsample ? 1 : 0; p.stride = stride;
   p.f8 = a->f8 ? 1 : 0;
   FEMASR_CHECK_ARG(!a->f8 || a->slice_kb == 0, "tc_igemm: the F8 cross-term mode is for the layers behind the VQ (no K slicing)");
+  FEMASR_CHECK_ARG(!a->f8 || (a->ksize != 4 && a->act != FEMASR_ACT_LRELU), "tc_igemm: no F8 cross-term mode for 4x4 convs or LeakyReLU");
   const TilePlan plan = plan_tiles(a, H, W);
   p.Wt = plan.Wt; p.Ht = plan.Ht; p.wt_shift = plan.wt_shift; p.tiles_x = plan.tiles_x; p.tiles_y = plan.tiles_y;
   const int BN = plan.BN;

@@ -11,9 +11,9 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("FEMASR_LIB") or os.path.join(_HERE, "libfemasr_b200.so")
 
-PRO_NONE, PRO_GN_SILU, PRO_LN, PRO_GN_SILU_FAST, PRO_MAXPOOL2 = 0, 1, 2, 3, 4
+PRO_NONE, PRO_GN_SILU, PRO_LN, PRO_GN_SILU_FAST, PRO_MAXPOOL2, PRO_BILINEAR2 = 0, 1, 2, 3, 4, 5
 ABI_VERSION = 4          # femasr_abi_version() of the library this binding was written against (include/femasr_b200.h)
-ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
+ACT_NONE, ACT_GELU, ACT_RELU, ACT_LRELU = 0, 1, 2, 3
 TAP_STAGES = ("in_conv", "down", "swin", "up1", "up2", "z", "zq", "after_quant", "dec0", "dec1", "dec2")
 SEMANTIC_TAP_STAGES = ("vgg", "semantic")      # only in a forward that computes the semantic loss
 
@@ -32,6 +32,10 @@ class NetConfig(C.Structure):
     _fields_ = [("scale_factor", C.c_int), ("n_e", C.c_int), ("e_dim", C.c_int), ("in_channel", C.c_int),
                 ("use_quantize", C.c_int), ("use_residual", C.c_int), ("gemm_path", C.c_int),
                 ("n_codebooks", C.c_int), ("cb_scale", C.c_int * 3), ("cb_n_e", C.c_int * 3), ("cb_e_dim", C.c_int * 3)]
+
+
+class DiscConfig(C.Structure):
+    _fields_ = [("num_in_ch", C.c_int), ("num_feat", C.c_int), ("skip_connection", C.c_int), ("gemm_path", C.c_int)]
 
 
 class IgemmArgs(C.Structure):
@@ -125,6 +129,14 @@ SIGNATURES = {
     "femasr_out_conv3x3_mma": (_I, [_V, _V, _V, _V, _I, _I, _I, _I, _V]),
     "femasr_nchw_to_nhwc": (_I, [_V, _V, _I, _I, _I, _I, _V]),
     "femasr_nhwc_to_nchw": (_I, [_V, _V, _I, _I, _I, _I, _V]),
+    "femasr_out_conv3x3_n": (_I, [_V, _V, _V, _V, _I, _I, _I, _I, _I, _I, _V]),
+    "femasr_spectral_sigma": (_I, [_V, _V, _V, _I, _I, _V, _V]),
+    "femasr_spectral_normalize": (_I, [_V, _V, _V, _Z, _V]),
+    "femasr_bilinear_up2": (_I, [_V, _V, _I, _I, _I, _I, _V]),
+    "femasr_disc_create": (_I, [C.POINTER(DiscConfig), C.POINTER(_V)]),
+    "femasr_disc_workspace_bytes": (_I, [_V, _I, _I, _I, C.POINTER(_Z)]),
+    "femasr_disc_forward": (_I, [_V, _V, _V, _I, _I, _I, _V, _Z, _V]),
+    "femasr_disc_flops": (_D, [_V, _I, _I, _I]),
 }
 
 _lib = None

@@ -4,7 +4,7 @@ arithmetic happens in libfemasr_b200.so through the C ABI (include/femasr_b200.h
 
 Mirrors the reference operator surface for this path (femasr_arch.py:311-479):
 encode_and_decode/forward -> NativeNet.forward, test -> NativeNet.test, test_tile -> NativeNet.test_tile,
-decode_indices -> NativeNet.decode_indices.
+decode_indices -> NativeNet.decode_indices; UNetDiscriminatorSN.forward (discriminator_arch.py) -> NativeDisc.forward.
 """
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from . import lib as L
-from .spec import normalize_codebooks, param_spec
+from .spec import disc_spec, normalize_codebooks, param_spec
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -48,7 +48,79 @@ def padded_size(n: int, scale: int) -> int:
     return (n // wsz + 1) * wsz
 
 
-class NativeNet:
+class _Engine:
+    """What every engine handle shares: creation on first use on a CUDA device, the parameter upload by reference name,
+    the device workspace and the per-kernel profile.  Subclasses set ``lib``, ``_h``, ``_ws``, ``device``, ``names``
+    and implement ``_create``."""
+
+    def _create(self):
+        raise NotImplementedError
+
+    # ------------------------------------------------------------------ lifecycle
+    def _ensure(self, device: torch.device):
+        if device.type != "cuda":
+            raise L.FemasrError("femasr_b200 runs on a CUDA sm_90 (H100) device only (no CPU fallback); "
+                                f"got tensors on '{device}'")
+        if self._h.value is None:
+            with torch.cuda.device(device):
+                L.require_device()
+                self._create()
+            self.device = device
+        elif device != self.device:
+            raise L.FemasrError(f"engine lives on {self.device}, input is on {device}")
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h.value is not None:
+            self.lib.femasr_net_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def load_state_dict(self, sd: Dict[str, torch.Tensor], device: torch.device):
+        """Upload every float parameter by its reference name (engine keeps repacked device copies)."""
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        self._ensure(device)
+        with torch.cuda.device(device):
+            for name in self.names:
+                if name not in sd:
+                    raise L.FemasrError(f"state_dict is missing '{name}'")
+                t = sd[name].detach()
+                if t.dtype != torch.float32:
+                    t = t.float()
+                t = t.contiguous()
+                on_dev = t.device.type == "cuda"
+                if on_dev and t.device != device:
+                    t = t.to(device)
+                L.check(self.lib.femasr_net_set_param(self._h, name.encode(), t.data_ptr(), t.numel(),
+                                                      int(on_dev), _stream()))
+            L.check(self.lib.femasr_net_params_complete(self._h))
+            torch.cuda.current_stream().synchronize()
+
+    def _workspace(self, nbytes: int) -> torch.Tensor:
+        if self._ws is None or self._ws.numel() < nbytes:
+            self._ws = None
+            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        return self._ws
+
+    def set_profile(self, enable: bool):
+        L.check(self.lib.femasr_net_set_profile(self._h, int(enable)))
+
+    def profile(self) -> dict:
+        """{kernel: {launches, ms, flops}} of the launches since set_profile(True) (CUDA-event timed)."""
+        import json
+        return json.loads(self.lib.femasr_net_profile_json(self._h).decode())
+
+    def last_launch_count(self) -> int:
+        return int(self.lib.femasr_net_last_launch_count(self._h))
+
+
+class NativeNet(_Engine):
     def __init__(self, scale_factor: int, n_e: int, e_dim: int, use_quantize: bool = True,
                  use_residual: bool = True, gemm_path: int = 0, codebooks=None, use_semantic_loss: bool = False):
         """``codebooks``: the reference's ``codebook_params`` rows [[scale, n_e, e_dim], ...] for the multi-scale
@@ -82,60 +154,14 @@ class NativeNet:
         self._seen_shapes: "OrderedDict[Tuple[int, ...], int]" = OrderedDict()
         self.last_from_graph = False     # whether the last forward_graph() result lives in a graph's static buffers
 
-    # ------------------------------------------------------------------ lifecycle
-    def _ensure(self, device: torch.device):
-        if device.type != "cuda":
-            raise L.FemasrError("femasr_b200 runs on a CUDA sm_90 (H100) device only (no CPU fallback); "
-                                f"got tensors on '{device}'")
-        if self._h.value is None:
-            with torch.cuda.device(device):
-                L.require_device()
-                L.check(self.lib.femasr_net_create(C.byref(self.cfg), C.byref(self._h)))
-                if self.use_semantic_loss:
-                    L.check(self.lib.femasr_net_enable_semantic(self._h))
-            self.device = device
-        elif device != self.device:
-            raise L.FemasrError(f"engine lives on {self.device}, input is on {device}")
-
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h.value is not None:
-            self.lib.femasr_net_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def _create(self):
+        L.check(self.lib.femasr_net_create(C.byref(self.cfg), C.byref(self._h)))
+        if self.use_semantic_loss:
+            L.check(self.lib.femasr_net_enable_semantic(self._h))
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor], device: torch.device):
-        """Upload every float parameter by its reference name (engine keeps repacked device copies)."""
         self._graphs.clear()           # captured graphs hold the old weight pointers' contents only by address: re-capture
-        device = torch.device(device)
-        if device.type == "cuda" and device.index is None:
-            device = torch.device("cuda", torch.cuda.current_device())
-        self._ensure(device)
-        with torch.cuda.device(device):
-            for name in self.names:
-                if name not in sd:
-                    raise L.FemasrError(f"state_dict is missing '{name}'")
-                t = sd[name].detach()
-                if t.dtype != torch.float32:
-                    t = t.float()
-                t = t.contiguous()
-                on_dev = t.device.type == "cuda"
-                if on_dev and t.device != device:
-                    t = t.to(device)
-                L.check(self.lib.femasr_net_set_param(self._h, name.encode(), t.data_ptr(), t.numel(),
-                                                      int(on_dev), _stream()))
-            L.check(self.lib.femasr_net_params_complete(self._h))
-            torch.cuda.current_stream().synchronize()
-
-    def _workspace(self, nbytes: int) -> torch.Tensor:
-        if self._ws is None or self._ws.numel() < nbytes:
-            self._ws = None
-            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        return self._ws
+        super().load_state_dict(sd, device)
 
     # ------------------------------------------------------------------ graph entry points
     def index_shapes(self, B: int, H: int, W: int) -> List[Tuple[int, int, int, int]]:
@@ -289,17 +315,6 @@ class NativeNet:
             if lo < 0 or hi >= n_e:
                 raise L.FemasrError(f"{what}: codebook index out of range [0, {n_e}): min {lo}, max {hi}")
 
-    def set_profile(self, enable: bool):
-        L.check(self.lib.femasr_net_set_profile(self._h, int(enable)))
-
-    def profile(self) -> dict:
-        """{kernel: {launches, ms, flops}} of the launches since set_profile(True) (CUDA-event timed)."""
-        import json
-        return json.loads(self.lib.femasr_net_profile_json(self._h).decode())
-
-    def last_launch_count(self) -> int:
-        return int(self.lib.femasr_net_last_launch_count(self._h))
-
     def flops(self, B: int, H: int, W: int) -> float:
         return float(self.lib.femasr_net_flops(self._h, B, H, W))
 
@@ -376,3 +391,36 @@ class NativeNet:
                                                             cy * s, cx * s, y0 * s, x0 * s, (y1 - y0) * s,
                                                             (x1 - x0) * s, st))
         return out
+
+
+class NativeDisc(_Engine):
+    """UNetDiscriminatorSN (discriminator_arch.py) on the engine: forward(x [B,3,H,W]) -> [B,1,H,W], eval mode."""
+
+    def __init__(self, skip_connection: bool = True, gemm_path: int = 0, num_in_ch: int = 3, num_feat: int = 64):
+        self.lib = L.load()
+        self.dcfg = L.DiscConfig(int(num_in_ch), int(num_feat), int(bool(skip_connection)), int(gemm_path))
+        self._h = C.c_void_p()
+        self._ws: Optional[torch.Tensor] = None
+        self.device: Optional[torch.device] = None
+        self.names = [n for (n, _s, _k, _f) in disc_spec(num_in_ch, num_feat)]
+
+    def _create(self):
+        L.check(self.lib.femasr_disc_create(C.byref(self.dcfg), C.byref(self._h)))
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        if x.dim() != 4 or x.shape[1] != self.dcfg.num_in_ch:
+            raise L.FemasrError(f"expected input [B,{self.dcfg.num_in_ch},H,W], got {tuple(x.shape)}")
+        self._ensure(x.device)
+        x = x.detach().float().contiguous()
+        B, _, H, W = x.shape
+        with torch.cuda.device(self.device):
+            y = torch.empty((B, 1, H, W), dtype=torch.float32, device=self.device)
+            need = C.c_size_t()
+            L.check(self.lib.femasr_disc_workspace_bytes(self._h, B, H, W, C.byref(need)))
+            ws = self._workspace(need.value)
+            L.check(self.lib.femasr_disc_forward(self._h, x.data_ptr(), y.data_ptr(), B, H, W, ws.data_ptr(), ws.numel(),
+                                                 _stream()))
+        return y
+
+    def flops(self, B: int, H: int, W: int) -> float:
+        return float(self.lib.femasr_disc_flops(self._h, B, H, W))

@@ -217,6 +217,54 @@ def random_state_dict(scale: int, e_dim: int, seed: int = 0, init: str = "defaul
     return sd
 
 
+def disc_spec(num_in_ch: int = 3, num_feat: int = 64) -> List[Tuple[str, tuple, str, int]]:
+    """UNetDiscriminatorSN's 28 state_dict tensors (discriminator_arch.py): conv0 / conv9 weight + bias, and for the
+    spectral_norm convs conv1 ... conv8 weight_orig [Cout,Cin,k,k], weight_u [Cout], weight_v [Cin*k*k].
+    kind: w | b (kaiming-uniform, fan_in), sn_w (weight_orig), sn_u | sn_v (fan_in carries their length)."""
+    F = num_feat
+    convs = [("conv1", F, 2 * F, 4), ("conv2", 2 * F, 4 * F, 4), ("conv3", 4 * F, 8 * F, 4), ("conv4", 8 * F, 4 * F, 3),
+             ("conv5", 4 * F, 2 * F, 3), ("conv6", 2 * F, F, 3), ("conv7", F, F, 3), ("conv8", F, F, 3)]
+    spec = _conv("conv0", num_in_ch, F, 3)
+    for name, ci, co, k in convs:
+        spec += [(f"{name}.weight_orig", (co, ci, k, k), "sn_w", ci * k * k), (f"{name}.weight_u", (co,), "sn_u", co),
+                 (f"{name}.weight_v", (ci * k * k,), "sn_v", ci * k * k)]
+    return spec + _conv("conv9", F, 1, 3)
+
+
+def power_iterate(w: torch.Tensor, u: torch.Tensor, v: torch.Tensor, n: int):
+    """n steps of torch.nn.utils.spectral_norm's power iteration on W = w.reshape(Cout, -1) (v = normalize(W^T u),
+    u = normalize(W v)), in fp64."""
+    wm = w.double().reshape(w.shape[0], -1)
+    u, v = u.double(), v.double()
+    for _ in range(n):
+        v = torch.nn.functional.normalize(wm.t() @ u, dim=0, eps=1e-12)
+        u = torch.nn.functional.normalize(wm @ v, dim=0, eps=1e-12)
+    return u.float(), v.float()
+
+
+def random_disc_state_dict(seed: int = 0, power_iterations: int = 30) -> Dict[str, torch.Tensor]:
+    """Seeded UNetDiscriminatorSN weights: conv weights and biases U(+-1/sqrt(fan_in)) like nn.Conv2d's default init, u
+    and v drawn like torch's spectral_norm (normalize(randn)) and then power-iterated ``power_iterations`` times in fp64,
+    which is what a trained checkpoint carries (the training-mode forward iterates once per step).  power_iterations=0
+    gives the never-iterated u, v of a freshly constructed network."""
+    sd: Dict[str, torch.Tensor] = {}
+    for name, shape, kind, fan_in in disc_spec():
+        g = _gen(seed, name)
+        if kind in ("w", "b", "sn_w"):
+            t = (torch.rand(shape, generator=g) * 2 - 1) / math.sqrt(fan_in)
+        elif kind in ("sn_u", "sn_v"):
+            t = torch.nn.functional.normalize(torch.randn(shape, generator=g), dim=0, eps=1e-12)
+        else:
+            raise ValueError(kind)
+        sd[name] = t.contiguous()
+    for name, _shape, kind, _f in disc_spec():
+        if kind == "sn_w" and power_iterations:
+            p = name[: -len(".weight_orig")]
+            sd[f"{p}.weight_u"], sd[f"{p}.weight_v"] = power_iterate(sd[name], sd[f"{p}.weight_u"], sd[f"{p}.weight_v"],
+                                                                      power_iterations)
+    return sd
+
+
 def vgg_init(shape, kind: str, fan_out: int, g: torch.Generator = None, init: str = "default") -> torch.Tensor:
     """VGG extractor tensors: torchvision's VGG init (kaiming-normal fan_out / relu: N(0, 2 / fan_out), bias 0; biases
     N(0, 0.01^2) for ``init='perturbed'``) and the ImageNet mean / std buffers."""

@@ -159,11 +159,17 @@ enum { FEMASR_PRO_NONE = 0, FEMASR_PRO_GN_SILU = 1, FEMASR_PRO_LN = 2,
        FEMASR_PRO_GN_SILU_FAST = 3,
        /* femasr_tc_prepare only: 2x2 stride-2 max-pool (nn.MaxPool2d(2, 2), floor) of the fp32 input before the split;
           H, W are the INPUT dims and a_hi/a_lo are [B,H/2,W/2,C] */
-       FEMASR_PRO_MAXPOOL2 = 4 };
-enum { FEMASR_ACT_NONE = 0, FEMASR_ACT_GELU = 1, FEMASR_ACT_RELU = 2 /* bias first, then max(v, 0) */ };
+       FEMASR_PRO_MAXPOOL2 = 4,
+       /* femasr_tc_prepare only: bilinear x2 upsample (F.interpolate(scale_factor=2, mode='bilinear',
+          align_corners=False)) of the fp32 input before the split; H, W are the INPUT dims and a_hi/a_lo are
+          [B,2H,2W,C] */
+       FEMASR_PRO_BILINEAR2 = 5 };
+enum { FEMASR_ACT_NONE = 0, FEMASR_ACT_GELU = 1, FEMASR_ACT_RELU = 2 /* bias first, then max(v, 0) */,
+       FEMASR_ACT_LRELU = 3 /* bias first, then v > 0 ? v : 0.2 * v (F.leaky_relu(negative_slope=0.2)) */ };
 
 /* Implicit-GEMM convolution / linear:  y = act(conv(pro(x)) + bias) + res1 + res2.
  *   ksize 3 (pad 1) or 1 (pad 0); stride 1|2; upsample=1 applies nearest x2 to pro(x) first
+ *   ksize 4 (pad 1) with stride 2 and no upsample: y is [B,(Hin+2-4)/2+1,(Win+2-4)/2+1,Cout]
  *   (nn.Upsample, femasr_arch.py:172,202).  Linear layers are ksize=1 with Hin*Win = tokens.
  *   prologue GN_SILU: x' = silu(x*pro_scale[b,c] + pro_shift[b,c])   (tables from femasr_gn_stats)
  *   prologue LN:      x' = (x - row_mean[m])*row_rstd[m]*gamma[c] + beta[c]
@@ -187,7 +193,7 @@ typedef struct {
 } femasr_igemm_args;
 int femasr_igemm_simt(const femasr_igemm_args* a, void* stream);
 
-/* ---- wgmma tensor-core implicit GEMM (gemm_path 1): same contract as femasr_igemm_simt for ksize 1|3,
+/* ---- wgmma tensor-core implicit GEMM (gemm_path 1): same contract as femasr_igemm_simt for ksize 1|3|4,
  * stride 1, Cin%64==0, Cout%64==0, computed as a 3-product split-fp16 GEMM (a_hi*w_hi + a_hi*w_lo + a_lo*w_hi,
  * fp32 accumulate in registers).  The activation operand is staged once per layer as two fp16 NHWC planes by
  * femasr_tc_prepare (which also applies the GN+SiLU / LayerNorm prologue and the nearest x2 upsample);
@@ -201,12 +207,13 @@ typedef struct {
   const float* res2;
   float* y;                /* fp32 NHWC [B,H,W,Cout] */
   int B, H, W, Cin, Cout;
-  int ksize;               /* 1 or 3 (pad 1) */
+  int ksize;               /* 1, 3 (pad 1) or 4 (pad 1, stride 2 only) */
   int act;                 /* FEMASR_ACT_* */
   void* out_hi;            /* optional: write the result as split fp16 NHWC planes (the next GEMM's operand) */
   void* out_lo;            /*           instead of fp32 y (y may then be NULL) */
   int stride;              /* 0|1: stride 1.  2: 3x3 stride-2 conv (pad 1); H,W are the INPUT dims, y is
-                              [B,(H-1)/2+1,(W-1)/2+1,Cout] (TMA traversal stride 2 on the activation planes) */
+                              [B,(H-1)/2+1,(W-1)/2+1,Cout] (TMA traversal stride 2 on the activation planes).
+                              ksize 4 (pad 1) requires stride 2: y is [B,(H+2-4)/2+1,(W+2-4)/2+1,Cout] */
   int kb_begin, kb_count;  /* K-slice in 64-wide k-blocks (k = tap*Cin + c); kb_count 0 = everything.  Slices are summed
                               by the caller in fp32 (round-to-nearest) by chaining launches with res1 = y, which bounds
                               the tensor-core accumulator's truncation error to one slice */
@@ -337,6 +344,8 @@ int femasr_in_conv_pad_weight(const float* w_oihw, float* w_padded, int Cout, vo
  * (x - mean[c]) / std[c] with a true fp32 division, and writes per pixel the 27 values of the 3x3 pad-1 window
  * (k = (kh*3+kw)*3+ci, zero padded to 64; the padding is zero AFTER normalisation like F.conv2d's) either as split fp16
  * planes a_hi/a_lo [B*H*W][64] (a_f32 NULL) or as fp32 rows a_f32 [B*H*W][64] (a_hi/a_lo NULL).
+ * mean == std_ == NULL: no normalisation, the rows hold the image values themselves (any other 3-channel 3x3 pad-1 conv,
+ * e.g. the discriminator's conv0); giving only one of the two is an error.
  * femasr_vgg_pad_weight: OIHW [Cout,3,3,3] -> [Cout][64] in that K order. */
 int femasr_vgg_im2col(const float* x_nchw, const float* mean, const float* std_, void* a_hi, void* a_lo, float* a_f32,
                       int B, int H, int W, void* stream);
@@ -356,6 +365,51 @@ int femasr_out_conv3x3(const float* x_nhwc, const float* w, const float* bias, f
  * (one engine handle = one host thread = one stream at a time, see the threading note in INTEGRATION.md). */
 int femasr_out_conv3x3_mma(const float* x_nhwc, const float* w, const float* bias, float* y_nchw, int B,
                            int H, int W, int Cin, void* stream);
+/* The same two kernels for a head of Cout = 3 (out_conv) or 1 (UNetDiscriminatorSN.conv9) output channels:
+ * NHWC [B,H,W,64] -> NCHW [B,Cout,H,W], w packed [9*64][Cout].  mma = 0: the SIMT kernel (femasr_out_conv3x3 for Cout 3);
+ * mma = 1: the tensor-core kernel (femasr_out_conv3x3_mma for Cout 3).  Same stream note as above. */
+int femasr_out_conv3x3_n(const float* x_nhwc, const float* w, const float* bias, float* y_nchw, int B, int H, int W,
+                         int Cin, int Cout, int mma, void* stream);
+
+/* Spectral normalisation in eval mode (torch.nn.utils.spectral_norm, no power iteration): W = w [Cout][K] (the
+ * weight_orig tensor reshaped), u [Cout], v [K].  femasr_spectral_sigma writes out[0] = u . (W v) (= sigma) and
+ * out[1] = |W v|, accumulated in fp64 in a fixed order and rounded to fp32 (device, 2 floats).  After one power
+ * iteration u = W v / |W v|, so out[0] == out[1]; out[0] << out[1] means u, v were never iterated.
+ * femasr_spectral_normalize: w_sn[i] = w[i] / sigma[0] (fp32 division, like weight_orig / sigma). */
+int femasr_spectral_sigma(const float* w, const float* u, const float* v, int Cout, int K, float* out, void* stream);
+int femasr_spectral_normalize(const float* w, const float* sigma, float* w_sn, size_t n, void* stream);
+/* F.interpolate(scale_factor=2, mode='bilinear', align_corners=False) on fp32 NHWC: x [B,H,W,C] -> y [B,2H,2W,C], C a
+ * multiple of 8 (the gemm_path 0 form of FEMASR_PRO_BILINEAR2). */
+int femasr_bilinear_up2(const float* x, float* y, int B, int H, int W, int C, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * UNetDiscriminatorSN (discriminator_arch.py; network_d of the training configs) in eval mode:
+ *   x0 = lrelu(conv0(x)); x1..x3 = lrelu(4x4 stride-2 SN convs); x4..x6 = lrelu(SN conv3x3(bilinear_x2(.))) [+ x2, x1, x0];
+ *   out = conv9(lrelu(conv8(lrelu(conv7(x6)))))   (lrelu slope 0.2).
+ * The handle is a femasr_net: femasr_net_set_param / params_complete / set_profile / profile_json / last_launch_count /
+ * destroy work on it; the generator entry points (forward*, workspace_bytes*, decode*, set_tap, enable_semantic) return
+ * FEMASR_ERR_ARG on a discriminator handle (femasr_net_flops returns 0), and the femasr_disc_* ones on a generator handle.
+ * Parameters: conv0.{weight,bias}, convN.{weight_orig,weight_u,weight_v} for N = 1..8, conv9.{weight,bias}.  An SN
+ * layer's weight forms are packed from weight_orig / sigma once all three of its tensors are set (in any order), and
+ * again whenever one of them is set anew.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int num_in_ch;        /* 3 */
+  int num_feat;         /* 64 */
+  int skip_connection;  /* 0 | 1 */
+  int gemm_path;        /* 0 = fp32 SIMT implicit GEMM, 1 = wgmma split-fp16 tensor-core GEMM (K-sliced, no F8) */
+} femasr_disc_config;
+int femasr_disc_create(const femasr_disc_config* cfg, femasr_net** out);
+/* Bytes of device workspace femasr_disc_forward needs for a [B,num_in_ch,H,W] input; H, W multiples of 8, else
+ * FEMASR_ERR_ARG (the reference raises at the skip add). */
+int femasr_disc_workspace_bytes(femasr_net* net, int B, int H, int W, size_t* bytes);
+/* x_nchw [B,3,H,W] fp32 device -> y_nchw [B,1,H,W] fp32 device.  gemm_path 1 returns FEMASR_ERR_STATE, naming the layer,
+ * when a layer's u . (W v) < 0.5 |W v| (u, v never power-iterated: sigma is tiny and the activations overflow fp16);
+ * gemm_path 0 runs such weights. */
+int femasr_disc_forward(femasr_net* net, const float* x_nchw, float* y_nchw, int B, int H, int W, void* workspace,
+                        size_t workspace_bytes, void* stream);
+/* Algorithmic FLOPs (2*MAC; conv0 at K = 27) of one femasr_disc_forward, from a sizing run; 0 for a rejected geometry. */
+double femasr_disc_flops(femasr_net* net, int B, int H, int W);
 
 /* layout helpers for tests */
 int femasr_nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, void* stream);
