@@ -85,10 +85,12 @@ __device__ __forceinline__ float gelu_erf_fast_f(float v) {
   return fmaf(-0.5f * fabsf(v), q, fmaxf(v, 0.0f));
 }
 
-// 2x2 stride-2 max-pool of 8 consecutive channels (nn.MaxPool2d(2, 2), floor): element i of the pooled NHWC tensor
-// [B,H/2,W/2,C] in 8-channel units; returns the pooled tensor's element offset.  Max in window order (0,0),(0,1),(1,0),(1,1).
-__device__ __forceinline__ long pool2_max8(const float* __restrict__ x, long i, int H, int W, int C, float (&v)[8]) {
-  const int c8 = C / 8, Ho = H / 2, Wo = W / 2;
+// KxK stride-2 max-pool of 8 consecutive channels (nn.MaxPool2d(K, 2), floor; K = 2 for VGG, 3 for AlexNet): element i
+// of the pooled NHWC tensor [B,(H-K)/2+1,(W-K)/2+1,C] in 8-channel units; returns the pooled tensor's element offset.
+// Max in window order (row-major).
+template <int K>
+__device__ __forceinline__ long pool_max8(const float* __restrict__ x, long i, int H, int W, int C, float (&v)[8]) {
+  const int c8 = C / 8, Ho = (H - K) / 2 + 1, Wo = (W - K) / 2 + 1;
   const int cq = (int)(i % c8);
   const long pix = i / c8;
   const int ox = (int)(pix % Wo);
@@ -98,9 +100,9 @@ __device__ __forceinline__ long pool2_max8(const float* __restrict__ x, long i, 
 #pragma unroll
   for (int k = 0; k < 8; ++k) v[k] = -INFINITY;
 #pragma unroll
-  for (int dy = 0; dy < 2; ++dy)
+  for (int dy = 0; dy < K; ++dy)
 #pragma unroll
-    for (int dx = 0; dx < 2; ++dx) {
+    for (int dx = 0; dx < K; ++dx) {
       const float4* s = reinterpret_cast<const float4*>(x + ((b * H + 2 * oy + dy) * W + 2 * ox + dx) * C + cq * 8);
       const float4 a = __ldg(s), c = __ldg(s + 1);
       const float w[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w};

@@ -79,8 +79,8 @@ constexpr unsigned
   FORM_TC8 = 1u << 2,      // the same in the F8 cross-term packing (3x3 convs that may run behind the VQ)
   FORM_UP = 1u << 3,       // sub-pixel phase filters of a nearest-x2 -> conv3x3 site, split fp16
   FORM_UP8 = 1u << 4,      // the same in the F8 packing
-  FORM_IM2COL = 1u << 5,   // [Cout][64] zero-padded im2col matrix (in_conv, VGG conv1_1): split-fp16 blob on gemm_path 1,
-                           // K-major fp32 on gemm_path 0
+  FORM_IM2COL = 1u << 5,   // [Cout][kpad] zero-padded im2col matrix (in_conv, VGG conv1_1, AlexNet conv1; kpad = im2col_k):
+                           // split-fp16 blob on gemm_path 1, K-major fp32 on gemm_path 0
   FORM_RELB = 1u << 6,     // rel-pos table expanded to [8][64][64] (SIMT attention) and in the mma kernel's fragment order
   FORM_ESQ = 1u << 7;      // sum e^2 per codebook row
 
@@ -133,6 +133,8 @@ struct femasr_net {
   int sem_slice_kb = 0;                   // K-slice length of the semantic branch's GEMMs (FEMASR_SEM_SLICE_KB; study knob, 0 = one pass)
   bool disc = false;                      // femasr_disc_create: a UNetDiscriminatorSN (dcfg); cfg holds only gemm_path
   femasr_disc_config dcfg{};
+  bool lpips = false;                     // femasr_lpips_create: an LPIPS metric (lcfg); cfg holds only gemm_path
+  femasr_lpips_config lcfg{};
   std::vector<ProfRec> prof;
   std::string prof_json;
   ~femasr_net() {
@@ -142,6 +144,13 @@ struct femasr_net {
 };
 
 namespace femasr {
+
+// the generator's entry points refuse the discriminator and LPIPS handles
+static bool generator(const femasr_net* n) { return !n->disc && !n->lpips; }
+
+// width of the zero-padded im2col rows of a 3-channel first conv with k x k taps (3 k^2 values): 64, or 384 for
+// AlexNet's 11x11 conv1
+static int im2col_k(int k) { return k == 11 ? 384 : 64; }
 
 static int chan(int res) {
   switch (res) { case 8: case 16: case 32: case 64: return 256; case 128: return 128; case 256: return 64; case 512: return 32; }
@@ -153,8 +162,8 @@ enum Role { CONV, UP_CONV, IN_CONV, VGG_CONV, VGG_CONV1, DISC_CONV };
 
 static unsigned weight_forms(const femasr_net* n, Role r, int ci, int co, int k) {
   const bool tc = n->cfg.gemm_path == 1;
-  if (r == VGG_CONV1 || (r == IN_CONV && tc)) return FORM_KMAJOR | FORM_IM2COL;   // K = 27 / 48 zero-padded to 64
-  if (!tc || (k != 1 && k != 3 && k != 4) || ci % 64 || co % 64) return FORM_KMAJOR;
+  if (r == VGG_CONV1 || (r == IN_CONV && tc)) return FORM_KMAJOR | FORM_IM2COL;   // K = 27 / 48 -> 64, 363 -> 384
+  if (!tc || (k != 1 && k != 3 && k != 4 && k != 5) || ci % 64 || co % 64) return FORM_KMAJOR;
   unsigned f = FORM_KMAJOR | FORM_TC;
   if (n->f8_cross && k == 3 && r != VGG_CONV && r != DISC_CONV) f |= FORM_TC8;   // may run behind the VQ; the VGG and
                                                                                   // discriminator convs never use F8
@@ -223,12 +232,27 @@ static void build_spec(femasr_net* n) {
   }
 }
 
-// VGG19 features up to relu4_4 (vgg_arch.py:55-139 with layer_name_list ['relu4_4']): every conv is 3x3 pad 1 + ReLU,
-// a 2x2/2 max-pool sits in front of conv2_1, conv3_1 and conv4_1.
-static const char* const VGG_CONVS[12] = {"conv1_1", "conv1_2", "conv2_1", "conv2_2", "conv3_1", "conv3_2",
-                                          "conv3_3", "conv3_4", "conv4_1", "conv4_2", "conv4_3", "conv4_4"};
-static const int VGG_COUT[12] = {64, 64, 128, 128, 256, 256, 256, 256, 512, 512, 512, 512};
-static const bool VGG_POOL_BEFORE[12] = {false, false, true, false, true, false, false, false, true, false, false, false};
+// A VGG-style stack: every conv is 3x3 pad 1 + ReLU, some have a 2x2/2 max-pool in front; `tap`: the ReLU output is a
+// feature the caller consumes (besides the last conv's).
+struct VggLayer { const char* w; int cout; bool pool_before, tap; };
+// VGG19 features up to relu4_4 (vgg_arch.py:55-139 with layer_name_list ['relu4_4']), under vgg_feat_extractor.vgg_net.
+static const VggLayer VGG19_RELU4_4[12] = {
+    {"conv1_1", 64, false, false}, {"conv1_2", 64, false, false}, {"conv2_1", 128, true, false}, {"conv2_2", 128, false, false},
+    {"conv3_1", 256, true, false}, {"conv3_2", 256, false, false}, {"conv3_3", 256, false, false}, {"conv3_4", 256, false, false},
+    {"conv4_1", 512, true, false}, {"conv4_2", 512, false, false}, {"conv4_3", 512, false, false}, {"conv4_4", 512, false, false}};
+// LPIPS' VGG16 (torchvision vgg16().features to relu5_3 as the lpips package's net.slice{1..5}.{i}); taps relu1_2, relu2_2,
+// relu3_3, relu4_3, relu5_3
+static const VggLayer VGG16_LPIPS[13] = {
+    {"net.slice1.0", 64, false, false},  {"net.slice1.2", 64, false, true},
+    {"net.slice2.5", 128, true, false},  {"net.slice2.7", 128, false, true},
+    {"net.slice3.10", 256, true, false}, {"net.slice3.12", 256, false, false}, {"net.slice3.14", 256, false, true},
+    {"net.slice4.17", 512, true, false}, {"net.slice4.19", 512, false, false}, {"net.slice4.21", 512, false, true},
+    {"net.slice5.24", 512, true, false}, {"net.slice5.26", 512, false, false}, {"net.slice5.28", 512, false, true}};
+// LPIPS' AlexNet (torchvision alexnet().features): the five convs (Cin, Cout, k); the ReLU after each is a tap
+struct AlexLayer { const char* w; int cin, cout, k; };
+static const AlexLayer ALEX_LPIPS[5] = {{"net.slice1.0", 3, 64, 11}, {"net.slice2.3", 64, 192, 5}, {"net.slice3.6", 192, 384, 3},
+                                        {"net.slice4.8", 384, 256, 3}, {"net.slice5.10", 256, 256, 3}};
+static const int LPIPS_TAP_C[2][5] = {{64, 192, 384, 256, 256}, {64, 128, 256, 512, 512}};   // [alex, vgg][tap]
 
 // use_semantic_loss=True (femasr_arch.py:301-309): conv_semantic = Sequential(Conv2d(512, 512, 1), ReLU) and the extractor
 static void add_semantic(femasr_net* n) {
@@ -237,9 +261,28 @@ static void add_semantic(femasr_net* n) {
   add_vec(n, "vgg_feat_extractor.std", 3);
   int cin = 3;
   for (int i = 0; i < 12; ++i) {
-    add_conv(n, std::string("vgg_feat_extractor.vgg_net.") + VGG_CONVS[i], cin, VGG_COUT[i], 3, i == 0 ? VGG_CONV1 : VGG_CONV);
-    cin = VGG_COUT[i];
+    const VggLayer& l = VGG19_RELU4_4[i];
+    add_conv(n, std::string("vgg_feat_extractor.vgg_net.") + l.w, cin, l.cout, 3, i == 0 ? VGG_CONV1 : VGG_CONV);
+    cin = l.cout;
   }
+}
+
+// LPIPS v0.1 (lpips package): the ScalingLayer buffers, the backbone convs and the five lin weights [1,C,1,1]
+static void build_lpips_spec(femasr_net* n) {
+  add_vec(n, "scaling_layer.shift", 3);
+  add_vec(n, "scaling_layer.scale", 3);
+  const bool vgg = n->lcfg.net == 1;
+  if (vgg) {
+    int cin = 3;
+    for (int i = 0; i < 13; ++i) {
+      add_conv(n, VGG16_LPIPS[i].w, cin, VGG16_LPIPS[i].cout, 3, i == 0 ? VGG_CONV1 : VGG_CONV);
+      cin = VGG16_LPIPS[i].cout;
+    }
+  } else {
+    for (int i = 0; i < 5; ++i)   // conv1: im2col GEMM, K = 363 -> 384
+      add_conv(n, ALEX_LPIPS[i].w, ALEX_LPIPS[i].cin, ALEX_LPIPS[i].cout, ALEX_LPIPS[i].k, i == 0 ? VGG_CONV1 : VGG_CONV);
+  }
+  for (int k = 0; k < 5; ++k) add_vec(n, "lin" + std::to_string(k) + ".model.1.weight", LPIPS_TAP_C[vgg][k]);
 }
 
 // UNetDiscriminatorSN (discriminator_arch.py): conv0 and conv9 plain convs with bias; conv1 ... conv8 spectral_norm convs
@@ -580,56 +623,143 @@ struct Ctx {
   }
 
   // vgg_feat = relu4_4((x - mean) / std) (femasr_arch.py:318-320).  Runs before the encoder: relu4_4 is allocated first
-  // and every full-resolution VGG buffer is released before the encoder's peak.  gemm_path 1 hands the activations from
-  // conv to conv as split fp16 planes; the pools read fp32 (pooling before the split) and write the next conv's planes.
-  // Every conv is bias + ReLU: the 3-product split-fp16 wgmma GEMM on gemm_path 1, the fp32 SIMT GEMM on gemm_path 0.
+  // and every full-resolution VGG buffer is released before the encoder's peak.
   void semantic_vgg(const float* x_nchw, int B, int H, int W) {
     const bool tc = net->cfg.gemm_path == 1;
-    const std::string pre = "vgg_feat_extractor.vgg_net.";
     vgg_feat = ar.alloc((size_t)B * (H / 8) * (W / 8) * 512);
+    float *ahi = nullptr, *alo = nullptr, *af = nullptr;   // conv1_1's operand: split planes (tc) or fp32
+    const size_t rows = (size_t)B * H * W;
+    if (tc) { ahi = ar.alloc(rows * 32); alo = ar.alloc(rows * 32); } else { af = ar.alloc(rows * 64); }
+    const float *mean = P("vgg_feat_extractor.mean"), *sd = P("vgg_feat_extractor.std");
+    run("vgg_im2col", 0.0, [&] { return femasr_vgg_im2col(x_nchw, mean, sd, ahi, alo, af, B, H, W, st); });
+    vgg_stack(VGG19_RELU4_4, 12, "vgg_feat_extractor.vgg_net.", "vgg_conv", "vgg_pool", B, H, W, ahi, alo, af, vgg_feat,
+              [](const float*, int, int, int) {});
+    tap("vgg", vgg_feat, (size_t)B * (H / 8) * (W / 8) * 512);
+  }
+
+  // The convs of a VggLayer table over B images of H x W, from conv 0's im2col operand (K = 27 -> 64: split planes ahi/alo
+  // on gemm_path 1, fp32 rows af on gemm_path 0), which this releases.  gemm_path 1 hands the activations from conv to
+  // conv as split fp16 planes; the pools read fp32 (pooling before the split) and write the next conv's planes.  Every
+  // conv is bias + ReLU: the 3-product split-fp16 wgmma GEMM on gemm_path 1, the fp32 SIMT GEMM on gemm_path 0.
+  // on_tap(f, h, w, c) sees the fp32 output of every tap layer while it is alive.  The last conv writes into `last` if
+  // given, else into an arena buffer that is returned for the caller to release.
+  template <class F>
+  float* vgg_stack(const VggLayer* L, int nl, const std::string& pre, const char* conv_name, const char* pool_name, int B,
+                   int H, int W, float* ahi, float* alo, float* af, float* last, F&& on_tap) {
+    const bool tc = net->cfg.gemm_path == 1;
     int h = H, w = W, c = 64;
-    float *ahi = nullptr, *alo = nullptr, *af = nullptr;   // the current conv's operand: split planes (tc) or fp32
-    {
-      const size_t rows = (size_t)B * H * W;
-      if (tc) { ahi = ar.alloc(rows * 32); alo = ar.alloc(rows * 32); } else { af = ar.alloc(rows * 64); }
-      const float *mean = P("vgg_feat_extractor.mean"), *sd = P("vgg_feat_extractor.std");
-      run("vgg_im2col", 0.0, [&] { return femasr_vgg_im2col(x_nchw, mean, sd, ahi, alo, af, B, H, W, st); });
-    }
     float* f = nullptr;                                    // fp32 output in front of a pool
-    for (int i = 0; i < 12; ++i) {
-      const int co = VGG_COUT[i];
-      if (VGG_POOL_BEFORE[i]) {
+    float* y = nullptr;
+    for (int i = 0; i < nl; ++i) {
+      const int co = L[i].cout;
+      if (L[i].pool_before) {
         const size_t n2 = (size_t)B * (h / 2) * (w / 2) * c;
         if (tc) {
           ahi = ar.alloc((n2 + 1) / 2); alo = ar.alloc((n2 + 1) / 2);
           const int hh = h, ww = w, cc = c;
-          run("vgg_pool", 0.0, [&] {
+          run(pool_name, 0.0, [&] {
             return femasr_tc_prepare(f, ahi, alo, FEMASR_PRO_MAXPOOL2, nullptr, nullptr, nullptr, nullptr, B, hh, ww, cc, 0, 0.f, st);
           });
         } else {
           af = ar.alloc(n2);
           const int hh = h, ww = w, cc = c;
-          run("vgg_pool", 0.0, [&] { return femasr_maxpool2(f, af, B, hh, ww, cc, st); });
+          run(pool_name, 0.0, [&] { return femasr_maxpool2(f, af, B, hh, ww, cc, st); });
         }
         ar.release(f); f = nullptr;
         h /= 2; w /= 2;
       }
-      const bool last = i == 11, to_f32 = !tc || last || VGG_POOL_BEFORE[i + 1];
+      const bool lastl = i == nl - 1, to_f32 = !tc || lastl || L[i].tap || L[i + 1].pool_before;
       const size_t n = (size_t)B * h * w * co;
-      float* y = last ? vgg_feat : (to_f32 ? ar.alloc(n) : nullptr);
+      y = lastl && last ? last : (to_f32 ? ar.alloc(n) : nullptr);
       float *ohi = nullptr, *olo = nullptr;
       if (!to_f32) { ohi = ar.alloc((n + 1) / 2); olo = ar.alloc((n + 1) / 2); }
-      // conv1_1: 1x1 GEMM over the K = 27 -> 64 im2col rows (27 algorithmic MACs)
-      ConvDesc g = geom(pre + VGG_CONVS[i], B, h, w, i == 0 ? 64 : c, co, i == 0 ? 1 : 3);
-      g.name = "vgg_conv"; g.semantic = true; g.im2col = i == 0; g.macs = i == 0 ? 27 : 0; g.act = FEMASR_ACT_RELU;
+      // conv 0: 1x1 GEMM over the K = 27 -> 64 im2col rows (27 algorithmic MACs)
+      ConvDesc g = geom(pre + L[i].w, B, h, w, i == 0 ? 64 : c, co, i == 0 ? 1 : 3);
+      g.name = conv_name; g.semantic = true; g.im2col = i == 0; g.macs = i == 0 ? 27 : 0; g.act = FEMASR_ACT_RELU;
       g.x = af; g.a_hi = ahi; g.a_lo = alo; g.y = y; g.o_hi = ohi; g.o_lo = olo;
       conv(g);
       if (tc) { ar.release(alo); ar.release(ahi); ahi = ohi; alo = olo; }
       else { ar.release(af); af = y; }
-      if (to_f32 && !last) f = y;
+      if (L[i].tap) on_tap(y, h, w, co);
+      if (to_f32 && !lastl) f = y;
       c = co;
     }
-    tap("vgg", vgg_feat, (size_t)B * h * w * 512);
+    return y;
+  }
+
+  // LPIPS v0.1 (lpips package, LPIPS.forward): d(x0, x1) for B pairs.  The backbone runs once over the 2B images [x0; x1]
+  // (the im2col writes x0's rows first, no concatenated copy); each tap's ReLU output goes through femasr_lpips_head while
+  // it is alive and is released as soon as the next layer has read it.  r [5][B] is per_layer, or workspace.  Numerics
+  // are those of the semantic loss's VGG convs: the 3-product split-fp16 GEMM without F8 on gemm_path 1, fp32 SIMT on 0.
+  void lpips(const float* x0, const float* x1, float* dist, float* per_layer, int B, int H, int W, int normalize) {
+    const bool tc = net->cfg.gemm_path == 1, vgg = net->lcfg.net == 1;
+    const int N = 2 * B;
+    float* r = per_layer ? per_layer : ar.alloc((size_t)5 * B);
+    int tap_k = 0;
+    auto head = [&](const float* f, int h, int w, int c) {
+      float* scratch = ar.alloc((femasr_lpips_head_scratch_bytes(B, h * w) + 3) / 4);
+      const float* lw = P("lin" + std::to_string(tap_k) + ".model.1.weight");
+      const int k = tap_k;
+      run("lpips_head", 0.0, [&] { return femasr_lpips_head(f, lw, B, h * w, c, r, k, k == 4 ? dist : nullptr, scratch, st); });
+      ar.release(scratch);
+      ++tap_k;
+    };
+    // first conv's operand: im2col of the scaled pair (vgg: 3x3 pad 1, K = 27 -> 64; alex: 11x11 stride 4 pad 2, K = 363 -> 384)
+    const int ks = vgg ? 3 : 11, stride = vgg ? 1 : 4, pad = vgg ? 1 : 2, kpad = im2col_k(ks);
+    const int h1 = (H + 2 * pad - ks) / stride + 1, w1 = (W + 2 * pad - ks) / stride + 1;
+    const size_t rows = (size_t)N * h1 * w1;
+    float *ahi = nullptr, *alo = nullptr, *af = nullptr;
+    if (tc) { ahi = ar.alloc(rows * kpad / 2); alo = ar.alloc(rows * kpad / 2); } else { af = ar.alloc(rows * kpad); }
+    const float *shift = P("scaling_layer.shift"), *scale = P("scaling_layer.scale");
+    run("lpips_im2col", 0.0, [&] {
+      return femasr_vgg_im2col_ex(x0, x1, B, H, W, ks, stride, pad, kpad, shift, scale, normalize, ahi, alo, af, st);
+    });
+    if (vgg) ar.release(vgg_stack(VGG16_LPIPS, 13, "", "lpips_conv", "lpips_pool", N, H, W, ahi, alo, af, nullptr, head));
+    else alex(ahi, alo, af, N, h1, w1, head);
+    if (!per_layer) ar.release(r);
+  }
+
+  // AlexNet features (torchvision): conv1 (the im2col GEMM) | pool 3/2, conv2 5x5 pad 2 | pool 3/2, conv3 | conv4 | conv5,
+  // each conv + ReLU and each ReLU a tap.  h, w: conv1's output size.  Releases conv1's operand.
+  template <class F>
+  void alex(float* ahi, float* alo, float* af, int N, int h, int w, F&& head) {
+    const bool tc = net->cfg.gemm_path == 1;
+    float* f = nullptr;                                    // the previous conv's fp32 output
+    for (int i = 0; i < 5; ++i) {
+      const AlexLayer& l = ALEX_LPIPS[i];
+      float *phi = nullptr, *plo = nullptr, *pf = nullptr;  // max-pool 3/2 output in front of conv2 and conv3
+      if (i == 1 || i == 2) {
+        const int hp = (h - 3) / 2 + 1, wp = (w - 3) / 2 + 1, hh = h, ww = w, cc = l.cin;
+        const size_t n2 = (size_t)N * hp * wp * l.cin;
+        const float* src = f;
+        if (tc) {
+          phi = ar.alloc((n2 + 1) / 2); plo = ar.alloc((n2 + 1) / 2);
+          run("lpips_pool", 0.0, [&] {
+            return femasr_tc_prepare(src, phi, plo, FEMASR_PRO_MAXPOOL3S2, nullptr, nullptr, nullptr, nullptr, N, hh, ww, cc, 0, 0.f, st);
+          });
+        } else {
+          pf = ar.alloc(n2);
+          run("lpips_pool", 0.0, [&] { return femasr_maxpool3s2(src, pf, N, hh, ww, cc, st); });
+        }
+        ar.release(f); f = nullptr;
+        h = hp; w = wp;
+      }
+      float* y = ar.alloc((size_t)N * h * w * l.cout);
+      // conv1: 1x1 GEMM over the K = 363 -> 384 im2col rows (363 algorithmic MACs)
+      ConvDesc g = geom(l.w, N, h, w, i == 0 ? im2col_k(l.k) : l.cin, l.cout, i == 0 ? 1 : l.k);
+      g.name = "lpips_conv"; g.semantic = true; g.act = FEMASR_ACT_RELU; g.y = y;
+      if (i == 0) { g.im2col = true; g.macs = 3 * l.k * l.k; g.x = af; g.a_hi = ahi; g.a_lo = alo; }
+      else if (phi) { g.a_hi = phi; g.a_lo = plo; }
+      else { g.x = pf ? pf : f; }
+      conv(g);
+      if (i == 0) { if (tc) { ar.release(alo); ar.release(ahi); } else { ar.release(af); } }
+      if (phi) { ar.release(plo); ar.release(phi); }
+      if (pf) ar.release(pf);
+      if (f) ar.release(f);
+      f = y;
+      head(f, h, w, l.cout);
+    }
+    ar.release(f);
   }
 
   // semantic_loss = mse(ReLU(conv_semantic(z_quant)), vgg_feat) (femasr_arch.py:344-347) on the quantiser's output
@@ -1044,15 +1174,16 @@ static int pack_forms(femasr_net* net, DevParam& d, const ParamInfo& pi, const f
   if ((f & FORM_KMAJOR) && ((s = ensure(&d.packed, pi.numel * sizeof(float))) || (s = femasr_pack_weight(src, d.packed, co, ci, k, k, st))))
     return s;
   if (f & FORM_IM2COL) {
-    // the im2col GEMM's weight: the [Cout][64] zero-padded matrix (K = 48 for in_conv, 27 for VGG conv1_1 and the
-    // discriminator's conv0), packed for this net's GEMM path
+    // the im2col GEMM's weight: the [Cout][kp] zero-padded matrix (K = 48 for in_conv, 27 for VGG conv1_1 and the
+    // discriminator's conv0, 363 for AlexNet's conv1), packed for this net's GEMM path
     const bool tc = net->cfg.gemm_path == 1;
+    const int kp = im2col_k(k);
     float* tmp = nullptr;
-    FEMASR_CUDA(cudaMallocAsync(&tmp, (size_t)co * 64 * sizeof(float), st));
-    s = k == 4 ? femasr_in_conv_pad_weight(src, tmp, co, st) : femasr_vgg_pad_weight(src, tmp, co, st);
-    if (!s) s = ensure(&d.im2col, tc ? femasr_tc_weight_bytes(co, 64, 1, 1) : (size_t)co * 64 * sizeof(float));
-    if (!s) s = tc ? femasr_tc_pack_weight(tmp, d.im2col, co, 64, 1, 1, st)
-                   : femasr_pack_weight(tmp, static_cast<float*>(d.im2col), co, 64, 1, 1, st);
+    FEMASR_CUDA(cudaMallocAsync(&tmp, (size_t)co * kp * sizeof(float), st));
+    s = k == 4 ? femasr_in_conv_pad_weight(src, tmp, co, st) : femasr_vgg_pad_weight_ex(src, tmp, co, k, kp, st);
+    if (!s) s = ensure(&d.im2col, tc ? femasr_tc_weight_bytes(co, kp, 1, 1) : (size_t)co * kp * sizeof(float));
+    if (!s) s = tc ? femasr_tc_pack_weight(tmp, d.im2col, co, kp, 1, 1, st)
+                   : femasr_pack_weight(tmp, static_cast<float*>(d.im2col), co, kp, 1, 1, st);
     cudaFreeAsync(tmp, st);
     if (s) return s;
   }
@@ -1098,7 +1229,7 @@ static int check_disc_geometry(int B, int H, int W) {
   return FEMASR_OK;
 }
 
-// Study knobs read from the environment at create time (generator and discriminator alike)
+// Study knobs read from the environment at create time (every kind of handle)
 static void read_knobs(femasr_net* n) {
   if (const char* ev = getenv("FEMASR_TC_PRECISE")) n->tc_precise = atoi(ev) != 0;
   if (const char* ev = getenv("FEMASR_FAST_SILU")) n->fast_silu = atoi(ev) != 0;
@@ -1161,7 +1292,7 @@ extern "C" void femasr_net_destroy(femasr_net* net) { delete net; }
 
 extern "C" int femasr_net_enable_semantic(femasr_net* net) {
   FEMASR_CHECK_ARG(net, "enable_semantic: null");
-  FEMASR_CHECK_ARG(!net->disc, "enable_semantic: a discriminator handle");
+  FEMASR_CHECK_ARG(generator(net), "enable_semantic: a discriminator or LPIPS handle");
   if (net->semantic) return FEMASR_OK;
   if (!net->dev.empty()) return fail(FEMASR_ERR_STATE, "enable_semantic: call it before the first set_param");
   add_semantic(net);
@@ -1196,13 +1327,13 @@ extern "C" int femasr_net_params_complete(femasr_net* net) {
 
 extern "C" int femasr_net_workspace_bytes(femasr_net* net, int B, int H, int W, size_t* bytes) {
   FEMASR_CHECK_ARG(net && bytes, "workspace_bytes: null pointer");
-  FEMASR_CHECK_ARG(!net->disc, "workspace_bytes: a discriminator handle (use femasr_disc_workspace_bytes)");
+  FEMASR_CHECK_ARG(generator(net), "workspace_bytes: a discriminator or LPIPS handle");
   return workspace_impl(net, B, H, W, false, bytes);
 }
 
 extern "C" int femasr_net_workspace_bytes_sem(femasr_net* net, int B, int H, int W, int with_sem, size_t* bytes) {
   FEMASR_CHECK_ARG(net && bytes, "workspace_bytes_sem: null pointer");
-  FEMASR_CHECK_ARG(!net->disc, "workspace_bytes_sem: a discriminator handle (use femasr_disc_workspace_bytes)");
+  FEMASR_CHECK_ARG(generator(net), "workspace_bytes_sem: a discriminator or LPIPS handle");
   return workspace_impl(net, B, H, W, with_sem != 0, bytes);
 }
 
@@ -1221,7 +1352,7 @@ extern "C" int femasr_net_forward_sem(femasr_net* net, const float* x, float* y,
                                       const int64_t* gt_indices, float* sem_loss, int B, int H, int W, void* workspace,
                                       size_t workspace_bytes, void* stream) {
   FEMASR_CHECK_ARG(net && x && y && workspace, "forward: null pointer");
-  FEMASR_CHECK_ARG(!net->disc, "forward: a discriminator handle (use femasr_disc_forward)");
+  FEMASR_CHECK_ARG(generator(net), "forward: a discriminator or LPIPS handle (use femasr_disc_forward / femasr_lpips_forward)");
   int s = check_geometry(net, B, H, W);
   if (s) return s;
   s = femasr_net_params_complete(net);
@@ -1238,7 +1369,7 @@ extern "C" int femasr_net_forward_sem(femasr_net* net, const float* x, float* y,
 
 extern "C" int femasr_net_decode_workspace_bytes(femasr_net* net, int B, int h, int w, size_t* bytes) {
   FEMASR_CHECK_ARG(net && bytes && B > 0 && h > 0 && w > 0, "decode_workspace_bytes: bad argument");
-  FEMASR_CHECK_ARG(!net->disc, "decode_workspace_bytes: a discriminator handle");
+  FEMASR_CHECK_ARG(generator(net), "decode_workspace_bytes: a discriminator or LPIPS handle");
   Ctx c(net, nullptr, 0, nullptr);
   c.decode_indices(nullptr, nullptr, B, h, w);
   *bytes = c.bytes_needed();
@@ -1248,7 +1379,7 @@ extern "C" int femasr_net_decode_workspace_bytes(femasr_net* net, int B, int h, 
 extern "C" int femasr_net_decode_indices(femasr_net* net, const int64_t* indices, float* y, int B, int h, int w,
                                          void* workspace, size_t workspace_bytes, void* stream) {
   FEMASR_CHECK_ARG(net && indices && y && workspace && B > 0 && h > 0 && w > 0, "decode_indices: bad argument");
-  FEMASR_CHECK_ARG(!net->disc, "decode_indices: a discriminator handle");
+  FEMASR_CHECK_ARG(generator(net), "decode_indices: a discriminator or LPIPS handle");
   int s = femasr_net_params_complete(net);
   if (s) return s;
   size_t need = 0;
@@ -1262,7 +1393,7 @@ extern "C" int femasr_net_decode_indices(femasr_net* net, const int64_t* indices
 
 extern "C" int femasr_net_set_tap(femasr_net* net, const char* stage, float* dst, size_t capacity) {
   FEMASR_CHECK_ARG(net && stage, "set_tap: null pointer");
-  FEMASR_CHECK_ARG(!net->disc, "set_tap: a discriminator handle");
+  FEMASR_CHECK_ARG(generator(net), "set_tap: a discriminator or LPIPS handle");
   static const char* names[] = {"in_conv", "down", "swin", "up1", "up2", "z", "zq", "after_quant", "dec0", "dec1", "dec2", "z1", "z2",
                                 "vgg", "semantic"};
   bool known = false;
@@ -1312,7 +1443,7 @@ extern "C" const char* femasr_net_profile_json(femasr_net* net) {
 // The sum of the algorithmic FLOPs the launches of one plain forward report (no taps, no gt_indices, no semantic loss),
 // counted by a sizing run; 0 for a geometry forward rejects.
 extern "C" double femasr_net_flops(femasr_net* net, int B, int H, int W) {
-  if (!net || net->disc || check_geometry(net, B, H, W)) return 0.0;
+  if (!net || !generator(net) || check_geometry(net, B, H, W)) return 0.0;
   std::map<std::string, Tap> taps;
   taps.swap(net->taps);          // a registered in_conv tap adds the fp32 in_conv to the tensor-core plan
   Ctx c(net, nullptr, 0, nullptr);
@@ -1341,7 +1472,7 @@ extern "C" int femasr_disc_create(const femasr_disc_config* cfg, femasr_net** ou
 
 extern "C" int femasr_disc_workspace_bytes(femasr_net* net, int B, int H, int W, size_t* bytes) {
   FEMASR_CHECK_ARG(net && bytes, "disc_workspace_bytes: null pointer");
-  FEMASR_CHECK_ARG(net->disc, "disc_workspace_bytes: a generator handle (use femasr_net_workspace_bytes)");
+  FEMASR_CHECK_ARG(net->disc, "disc_workspace_bytes: not a discriminator handle");
   int s = check_disc_geometry(B, H, W);
   if (s) return s;
   Ctx c(net, nullptr, 0, nullptr);
@@ -1353,7 +1484,7 @@ extern "C" int femasr_disc_workspace_bytes(femasr_net* net, int B, int H, int W,
 extern "C" int femasr_disc_forward(femasr_net* net, const float* x, float* y, int B, int H, int W, void* workspace,
                                    size_t workspace_bytes, void* stream) {
   FEMASR_CHECK_ARG(net && x && y && workspace, "disc_forward: null pointer");
-  FEMASR_CHECK_ARG(net->disc, "disc_forward: a generator handle (use femasr_net_forward)");
+  FEMASR_CHECK_ARG(net->disc, "disc_forward: not a discriminator handle");
   int s = check_disc_geometry(B, H, W);
   if (s) return s;
   s = femasr_net_params_complete(net);
@@ -1386,5 +1517,68 @@ extern "C" double femasr_disc_flops(femasr_net* net, int B, int H, int W) {
   if (!net || !net->disc || check_disc_geometry(B, H, W)) return 0.0;
   Ctx c(net, nullptr, 0, nullptr);
   c.disc(nullptr, nullptr, B, H, W);
+  return c.flops;
+}
+
+// ------------------------------------------------------------------------------------------------ LPIPS
+static int check_lpips_geometry(femasr_net* net, int B, int H, int W) {
+  if (B <= 0 || H <= 0 || W <= 0) return fail(FEMASR_ERR_ARG, "lpips: empty input");
+  const std::string got = " (got " + std::to_string(H) + "x" + std::to_string(W) + ")";
+  if (net->lcfg.net == 1 && (H % 16 || W % 16))
+    return fail(FEMASR_ERR_ARG, "lpips (vgg): H and W must be multiples of 16, so that each of the four 2x2 max-pools is exact" + got);
+  if (net->lcfg.net == 0 && (H < 31 || W < 31))
+    return fail(FEMASR_ERR_ARG, "lpips (alex): H and W must be at least 31, the smallest input AlexNet's features accept" + got);
+  return FEMASR_OK;
+}
+
+extern "C" int femasr_lpips_create(const femasr_lpips_config* cfg, femasr_net** out) {
+  FEMASR_CHECK_ARG(cfg && out, "lpips_create: null pointer");
+  FEMASR_CHECK_ARG(cfg->net == 0 || cfg->net == 1, "lpips_create: net must be 0 (alex) or 1 (vgg)");
+  FEMASR_CHECK_ARG(cfg->gemm_path == 0 || cfg->gemm_path == 1, "lpips_create: gemm_path must be 0 or 1");
+  femasr_net* n = new femasr_net();
+  n->cfg = femasr_net_config{};
+  n->cfg.gemm_path = cfg->gemm_path;
+  n->lpips = true;
+  n->lcfg = *cfg;
+  read_knobs(n);
+  build_lpips_spec(n);
+  *out = n;
+  return FEMASR_OK;
+}
+
+extern "C" int femasr_lpips_workspace_bytes(femasr_net* net, int B, int H, int W, size_t* bytes) {
+  FEMASR_CHECK_ARG(net && bytes, "lpips_workspace_bytes: null pointer");
+  FEMASR_CHECK_ARG(net->lpips, "lpips_workspace_bytes: not an LPIPS handle");
+  int s = check_lpips_geometry(net, B, H, W);
+  if (s) return s;
+  Ctx c(net, nullptr, 0, nullptr);
+  c.lpips(nullptr, nullptr, nullptr, nullptr, B, H, W, 0);
+  *bytes = c.bytes_needed();
+  return c.status;
+}
+
+extern "C" int femasr_lpips_forward(femasr_net* net, const float* x0, const float* x1, float* dist, float* per_layer, int B,
+                                    int H, int W, int normalize, void* workspace, size_t workspace_bytes, void* stream) {
+  FEMASR_CHECK_ARG(net && x0 && x1 && dist && workspace, "lpips_forward: null pointer");
+  FEMASR_CHECK_ARG(net->lpips, "lpips_forward: not an LPIPS handle");
+  int s = check_lpips_geometry(net, B, H, W);
+  if (s) return s;
+  s = femasr_net_params_complete(net);
+  if (s) return s;
+  size_t need = 0;
+  s = femasr_lpips_workspace_bytes(net, B, H, W, &need);
+  if (s) return s;
+  if (workspace_bytes < need) return fail(FEMASR_ERR_STATE, "lpips_forward: workspace too small (need " + std::to_string(need) + " bytes)");
+  Ctx c(net, workspace, workspace_bytes, stream);
+  c.lpips(x0, x1, dist, per_layer, B, H, W, normalize);
+  return c.finish();
+}
+
+// The sum of the algorithmic FLOPs of one femasr_lpips_forward's launches (both images of every pair), counted by a sizing
+// run; 0 for a rejected geometry or another kind of handle.
+extern "C" double femasr_lpips_flops(femasr_net* net, int B, int H, int W) {
+  if (!net || !net->lpips || check_lpips_geometry(net, B, H, W)) return 0.0;
+  Ctx c(net, nullptr, 0, nullptr);
+  c.lpips(nullptr, nullptr, nullptr, nullptr, B, H, W, 0);
   return c.flops;
 }

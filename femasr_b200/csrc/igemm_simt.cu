@@ -191,7 +191,12 @@ int igemm_out_dims(const femasr_igemm_args* a, int* Ho, int* Wo) {
     *Ho = (a->Hin + 2 - 4) / 2 + 1; *Wo = (a->Win + 2 - 4) / 2 + 1;
     return FEMASR_OK;
   }
-  if (a->ksize != 3) return fail(FEMASR_ERR_ARG, "igemm: ksize must be 1, 3 or 4");
+  if (a->ksize == 5) {      // 5x5 pad 2 stride 1 (AlexNet conv2 of LPIPS)
+    if (a->stride != 1 || a->upsample) return fail(FEMASR_ERR_ARG, "igemm: 5x5 supports stride 1, no upsample");
+    *Ho = a->Hin; *Wo = a->Win;
+    return FEMASR_OK;
+  }
+  if (a->ksize != 3) return fail(FEMASR_ERR_ARG, "igemm: ksize must be 1, 3, 4 or 5");
   const int He = a->upsample ? 2 * a->Hin : a->Hin, We = a->upsample ? 2 * a->Win : a->Win;
   if (a->stride == 1) { *Ho = He; *Wo = We; }
   else if (a->stride == 2) { *Ho = (He + 2 - 3) / 2 + 1; *Wo = (We + 2 - 3) / 2 + 1; }
@@ -215,7 +220,7 @@ extern "C" int femasr_igemm_simt(const femasr_igemm_args* a, void* stream) {
   p.x = a->x; p.w = a->w; p.bias = a->bias; p.res1 = a->res1; p.res2 = a->res2; p.y = a->y;
   p.pro_a = a->pro_a; p.pro_b = a->pro_b; p.gamma = a->gamma; p.beta = a->beta;
   p.B = a->B; p.Hin = a->Hin; p.Win = a->Win; p.Cin = a->Cin; p.Cout = a->Cout;
-  p.ksize = a->ksize; p.stride = a->stride; p.upsample = a->upsample; p.pad = a->ksize == 1 ? 0 : 1;
+  p.ksize = a->ksize; p.stride = a->stride; p.upsample = a->upsample; p.pad = a->ksize == 1 ? 0 : (a->ksize == 5 ? 2 : 1);
   p.act = a->act;
   p.M = (long)a->B * p.Ho * p.Wo;
   if (a->Cout % 128 == 0) return launch_bn<128>(p, a->prologue, as_stream(stream));

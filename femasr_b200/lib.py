@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("FEMASR_LIB") or os.path.join(_HERE, "libfemasr_b200.so")
 
-PRO_NONE, PRO_GN_SILU, PRO_LN, PRO_GN_SILU_FAST, PRO_MAXPOOL2, PRO_BILINEAR2 = 0, 1, 2, 3, 4, 5
+PRO_NONE, PRO_GN_SILU, PRO_LN, PRO_GN_SILU_FAST, PRO_MAXPOOL2, PRO_BILINEAR2, PRO_MAXPOOL3S2 = 0, 1, 2, 3, 4, 5, 6
 ABI_VERSION = 4          # femasr_abi_version() of the library this binding was written against (include/femasr_b200.h)
 ACT_NONE, ACT_GELU, ACT_RELU, ACT_LRELU = 0, 1, 2, 3
 TAP_STAGES = ("in_conv", "down", "swin", "up1", "up2", "z", "zq", "after_quant", "dec0", "dec1", "dec2")
@@ -36,6 +36,10 @@ class NetConfig(C.Structure):
 
 class DiscConfig(C.Structure):
     _fields_ = [("num_in_ch", C.c_int), ("num_feat", C.c_int), ("skip_connection", C.c_int), ("gemm_path", C.c_int)]
+
+
+class LpipsConfig(C.Structure):
+    _fields_ = [("net", C.c_int), ("gemm_path", C.c_int)]
 
 
 class IgemmArgs(C.Structure):
@@ -137,6 +141,15 @@ SIGNATURES = {
     "femasr_disc_workspace_bytes": (_I, [_V, _I, _I, _I, C.POINTER(_Z)]),
     "femasr_disc_forward": (_I, [_V, _V, _V, _I, _I, _I, _V, _Z, _V]),
     "femasr_disc_flops": (_D, [_V, _I, _I, _I]),
+    "femasr_vgg_im2col_ex": (_I, [_V, _V, _I, _I, _I, _I, _I, _I, _I, _V, _V, _I, _V, _V, _V, _V]),
+    "femasr_vgg_pad_weight_ex": (_I, [_V, _V, _I, _I, _I, _V]),
+    "femasr_maxpool3s2": (_I, [_V, _V, _I, _I, _I, _I, _V]),
+    "femasr_lpips_create": (_I, [C.POINTER(LpipsConfig), C.POINTER(_V)]),
+    "femasr_lpips_workspace_bytes": (_I, [_V, _I, _I, _I, C.POINTER(_Z)]),
+    "femasr_lpips_forward": (_I, [_V, _V, _V, _V, _V, _I, _I, _I, _I, _V, _Z, _V]),
+    "femasr_lpips_flops": (_D, [_V, _I, _I, _I]),
+    "femasr_lpips_head_scratch_bytes": (_Z, [_I, _I]),
+    "femasr_lpips_head": (_I, [_V, _V, _I, _I, _I, _V, _I, _V, _V, _V]),
 }
 
 _lib = None

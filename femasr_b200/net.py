@@ -4,7 +4,8 @@ arithmetic happens in libfemasr_b200.so through the C ABI (include/femasr_b200.h
 
 Mirrors the reference operator surface for this path (femasr_arch.py:311-479):
 encode_and_decode/forward -> NativeNet.forward, test -> NativeNet.test, test_tile -> NativeNet.test_tile,
-decode_indices -> NativeNet.decode_indices; UNetDiscriminatorSN.forward (discriminator_arch.py) -> NativeDisc.forward.
+decode_indices -> NativeNet.decode_indices; UNetDiscriminatorSN.forward (discriminator_arch.py) -> NativeDisc.forward;
+the lpips package's LPIPS.forward -> NativeLPIPS.forward.
 """
 from __future__ import annotations
 
@@ -17,7 +18,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from . import lib as L
-from .spec import disc_spec, normalize_codebooks, param_spec
+from .spec import disc_spec, lpips_spec, normalize_codebooks, param_spec
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -424,3 +425,42 @@ class NativeDisc(_Engine):
 
     def flops(self, B: int, H: int, W: int) -> float:
         return float(self.lib.femasr_disc_flops(self._h, B, H, W))
+
+
+class NativeLPIPS(_Engine):
+    """LPIPS v0.1 (the lpips package, net 'alex' | 'vgg') on the engine: forward(x0, x1) -> (d [B], r [5, B])."""
+
+    def __init__(self, net: str = "alex", gemm_path: int = 0):
+        self.lib = L.load()
+        self.net = net
+        self.lcfg = L.LpipsConfig({"alex": 0, "vgg": 1}[net], int(gemm_path))
+        self._h = C.c_void_p()
+        self._ws: Optional[torch.Tensor] = None
+        self.device: Optional[torch.device] = None
+        self.names = [n for (n, _s, _k, _f) in lpips_spec(net)]
+
+    def _create(self):
+        L.check(self.lib.femasr_lpips_create(C.byref(self.lcfg), C.byref(self._h)))
+
+    def forward(self, x0: torch.Tensor, x1: torch.Tensor, normalize: bool = False):
+        """x0, x1 [B,3,H,W] -> (d [B], per-layer r [5,B]) fp32 on the device."""
+        if x0.dim() != 4 or x0.shape[1] != 3 or x0.shape != x1.shape:
+            raise L.FemasrError(f"expected two inputs [B,3,H,W] of one shape, got {tuple(x0.shape)} and {tuple(x1.shape)}")
+        self._ensure(x0.device)
+        if x1.device != x0.device:
+            raise L.FemasrError(f"inputs on different devices: {x0.device} and {x1.device}")
+        x0 = x0.detach().float().contiguous()
+        x1 = x1.detach().float().contiguous()
+        B, _, H, W = x0.shape
+        with torch.cuda.device(self.device):
+            d = torch.empty(B, dtype=torch.float32, device=self.device)
+            r = torch.empty(5, B, dtype=torch.float32, device=self.device)
+            need = C.c_size_t()
+            L.check(self.lib.femasr_lpips_workspace_bytes(self._h, B, H, W, C.byref(need)))
+            ws = self._workspace(need.value)
+            L.check(self.lib.femasr_lpips_forward(self._h, x0.data_ptr(), x1.data_ptr(), d.data_ptr(), r.data_ptr(), B, H,
+                                                  W, int(bool(normalize)), ws.data_ptr(), ws.numel(), _stream()))
+        return d, r
+
+    def flops(self, B: int, H: int, W: int) -> float:
+        return float(self.lib.femasr_lpips_flops(self._h, B, H, W))

@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import hashlib
 import math
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -277,3 +277,52 @@ def vgg_init(shape, kind: str, fan_out: int, g: torch.Generator = None, init: st
     if kind == "vgg_std":
         return torch.tensor(VGG_STD).view(shape)
     raise ValueError(kind)
+
+
+# LPIPS v0.1 (the lpips package): torchvision features index, Cin, Cout, k of every backbone conv per slice, and the
+# channel count of each of the five taps (lin0 ... lin4)
+LPIPS_CONVS = {
+    "alex": [(1, 0, 3, 64, 11), (2, 3, 64, 192, 5), (3, 6, 192, 384, 3), (4, 8, 384, 256, 3), (5, 10, 256, 256, 3)],
+    "vgg": [(1, 0, 3, 64, 3), (1, 2, 64, 64, 3), (2, 5, 64, 128, 3), (2, 7, 128, 128, 3), (3, 10, 128, 256, 3),
+            (3, 12, 256, 256, 3), (3, 14, 256, 256, 3), (4, 17, 256, 512, 3), (4, 19, 512, 512, 3), (4, 21, 512, 512, 3),
+            (5, 24, 512, 512, 3), (5, 26, 512, 512, 3), (5, 28, 512, 512, 3)],
+}
+LPIPS_CHANNELS = {"alex": (64, 192, 384, 256, 256), "vgg": (64, 128, 256, 512, 512)}
+LPIPS_SHIFT = (-0.030, -0.088, -0.188)      # lpips.ScalingLayer buffers
+LPIPS_SCALE = (0.458, 0.448, 0.450)
+
+
+def lpips_spec(net: str) -> List[Tuple[str, tuple, str, int]]:
+    """The lpips package's LPIPS(net=net) state_dict, in its order: scaling_layer.{shift,scale} [1,3,1,1] (kind shift |
+    scale), net.slice{s}.{i}.{weight,bias} (kind w | b; fan_in Cin*k*k) with i the torchvision features index, and
+    lin{k}.model.1.weight [1,C,1,1] (kind lin, fan_in C)."""
+    if net not in LPIPS_CONVS:
+        raise ValueError(f"LPIPS net must be 'alex' or 'vgg', got {net!r}")
+    spec = [("scaling_layer.shift", (1, 3, 1, 1), "shift", 3), ("scaling_layer.scale", (1, 3, 1, 1), "scale", 3)]
+    for s, i, ci, co, k in LPIPS_CONVS[net]:
+        spec += _conv(f"net.slice{s}.{i}", ci, co, k)
+    spec += [(f"lin{k}.model.1.weight", (1, c, 1, 1), "lin", c) for k, c in enumerate(LPIPS_CHANNELS[net])]
+    return spec
+
+
+def random_lpips_state_dict(net: str, seed: Optional[int] = None) -> Dict[str, torch.Tensor]:
+    """Untrained LPIPS tensors: the ScalingLayer constants, the backbone as torchvision initialises it (alexnet: nn.Conv2d's
+    default U(+-1/sqrt(fan_in)) for weight and bias; vgg16: kaiming-normal fan_out / relu, bias 0) and non-negative lins
+    |N(0, 0.3^2)|, which put d in about 0.05 ... 1 like a trained LPIPS.  seed None: torch's global generator."""
+    g = None if seed is None else _gen(seed, "lpips-" + net)
+    out: Dict[str, torch.Tensor] = {}
+    for name, shape, kind, fan_in in lpips_spec(net):
+        if kind == "shift":
+            t = torch.tensor(LPIPS_SHIFT).view(shape)
+        elif kind == "scale":
+            t = torch.tensor(LPIPS_SCALE).view(shape)
+        elif kind == "lin":
+            t = torch.randn(shape, generator=g).abs() * 0.3
+        elif net == "alex":
+            t = (torch.rand(shape, generator=g) * 2 - 1) / math.sqrt(fan_in)
+        elif kind == "w":
+            t = torch.randn(shape, generator=g) * math.sqrt(2.0 / (shape[0] * shape[2] * shape[3]))
+        else:
+            t = torch.zeros(shape)
+        out[name] = t.contiguous()
+    return out

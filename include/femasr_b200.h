@@ -163,13 +163,17 @@ enum { FEMASR_PRO_NONE = 0, FEMASR_PRO_GN_SILU = 1, FEMASR_PRO_LN = 2,
        /* femasr_tc_prepare only: bilinear x2 upsample (F.interpolate(scale_factor=2, mode='bilinear',
           align_corners=False)) of the fp32 input before the split; H, W are the INPUT dims and a_hi/a_lo are
           [B,2H,2W,C] */
-       FEMASR_PRO_BILINEAR2 = 5 };
+       FEMASR_PRO_BILINEAR2 = 5,
+       /* femasr_tc_prepare only: 3x3 stride-2 max-pool (nn.MaxPool2d(3, 2), floor; AlexNet) of the fp32 input before the
+          split; H, W are the INPUT dims (>= 3) and a_hi/a_lo are [B,(H-3)/2+1,(W-3)/2+1,C] */
+       FEMASR_PRO_MAXPOOL3S2 = 6 };
 enum { FEMASR_ACT_NONE = 0, FEMASR_ACT_GELU = 1, FEMASR_ACT_RELU = 2 /* bias first, then max(v, 0) */,
        FEMASR_ACT_LRELU = 3 /* bias first, then v > 0 ? v : 0.2 * v (F.leaky_relu(negative_slope=0.2)) */ };
 
 /* Implicit-GEMM convolution / linear:  y = act(conv(pro(x)) + bias) + res1 + res2.
  *   ksize 3 (pad 1) or 1 (pad 0); stride 1|2; upsample=1 applies nearest x2 to pro(x) first
  *   ksize 4 (pad 1) with stride 2 and no upsample: y is [B,(Hin+2-4)/2+1,(Win+2-4)/2+1,Cout]
+ *   ksize 5 (pad 2) with stride 1 and no upsample: y is [B,Hin,Win,Cout]
  *   (nn.Upsample, femasr_arch.py:172,202).  Linear layers are ksize=1 with Hin*Win = tokens.
  *   prologue GN_SILU: x' = silu(x*pro_scale[b,c] + pro_shift[b,c])   (tables from femasr_gn_stats)
  *   prologue LN:      x' = (x - row_mean[m])*row_rstd[m]*gamma[c] + beta[c]
@@ -193,7 +197,7 @@ typedef struct {
 } femasr_igemm_args;
 int femasr_igemm_simt(const femasr_igemm_args* a, void* stream);
 
-/* ---- wgmma tensor-core implicit GEMM (gemm_path 1): same contract as femasr_igemm_simt for ksize 1|3|4,
+/* ---- wgmma tensor-core implicit GEMM (gemm_path 1): same contract as femasr_igemm_simt for ksize 1|3|4|5,
  * stride 1, Cin%64==0, Cout%64==0, computed as a 3-product split-fp16 GEMM (a_hi*w_hi + a_hi*w_lo + a_lo*w_hi,
  * fp32 accumulate in registers).  The activation operand is staged once per layer as two fp16 NHWC planes by
  * femasr_tc_prepare (which also applies the GN+SiLU / LayerNorm prologue and the nearest x2 upsample);
@@ -207,7 +211,7 @@ typedef struct {
   const float* res2;
   float* y;                /* fp32 NHWC [B,H,W,Cout] */
   int B, H, W, Cin, Cout;
-  int ksize;               /* 1, 3 (pad 1) or 4 (pad 1, stride 2 only) */
+  int ksize;               /* 1, 3 (pad 1), 4 (pad 1, stride 2 only) or 5 (pad 2, stride 1 only) */
   int act;                 /* FEMASR_ACT_* */
   void* out_hi;            /* optional: write the result as split fp16 NHWC planes (the next GEMM's operand) */
   void* out_lo;            /*           instead of fp32 y (y may then be NULL) */
@@ -350,8 +354,23 @@ int femasr_in_conv_pad_weight(const float* w_oihw, float* w_padded, int Cout, vo
 int femasr_vgg_im2col(const float* x_nchw, const float* mean, const float* std_, void* a_hi, void* a_lo, float* a_f32,
                       int B, int H, int W, void* stream);
 int femasr_vgg_pad_weight(const float* w_oihw, float* w_padded, int Cout, void* stream);
+/* The general form of the two (femasr_vgg_im2col is ksize 3, stride 1, pad 1, kpad 64, x1 NULL, no 2x-1 step):
+ *   x0, x1     [B,3,H,W] each; x1 may be NULL.  Rows of x0's images come first, then x1's: [2B*Ho*Wo][kpad] (or
+ *              [B*Ho*Wo][kpad] without x1), Ho = (H + 2 pad - ksize) / stride + 1, likewise Wo
+ *   window     ksize x ksize taps at the given stride and zero pad, k = (kh*ksize+kw)*3+ci, zero padded to kpad (a
+ *              multiple of 64, at least 3*ksize^2): AlexNet's conv1 of LPIPS is ksize 11, stride 4, pad 2, kpad 384
+ *   transform  two_x_minus_1: x' = 2x - 1 first (LPIPS normalize=True); then (x' - mean) / std as an fp32 division
+ *              when mean/std are given (LPIPS' ScalingLayer shift / scale)
+ * femasr_vgg_pad_weight_ex: OIHW [Cout,3,ksize,ksize] -> [Cout][kpad] in that K order. */
+int femasr_vgg_im2col_ex(const float* x0, const float* x1, int B, int H, int W, int ksize, int stride, int pad,
+                         int kpad, const float* mean, const float* std_, int two_x_minus_1, void* a_hi, void* a_lo,
+                         float* a_f32, void* stream);
+int femasr_vgg_pad_weight_ex(const float* w_oihw, float* w_padded, int Cout, int ksize, int kpad, void* stream);
 /* nn.MaxPool2d(2, 2) on fp32 NHWC: x [B,H,W,C] -> y [B,H/2,W/2,C] (the gemm_path 0 form of FEMASR_PRO_MAXPOOL2). */
 int femasr_maxpool2(const float* x, float* y, int B, int H, int W, int C, void* stream);
+/* nn.MaxPool2d(3, 2) (floor) on fp32 NHWC: x [B,H,W,C] -> y [B,(H-3)/2+1,(W-3)/2+1,C], H, W >= 3 (the gemm_path 0 form of
+ * FEMASR_PRO_MAXPOOL3S2). */
+int femasr_maxpool3s2(const float* x, float* y, int B, int H, int W, int C, void* stream);
 /* rows[i] = sum_c (a[i][c] - b[i][c])^2 over [N, C] fp32, in a fixed order (one warp per row); the mean is then
  * femasr_sum_scaled(rows, out, N, 1 / (N * C)). */
 int femasr_sq_diff_rows(const float* a, const float* b, float* rows, int N, int C, void* stream);
@@ -410,6 +429,44 @@ int femasr_disc_forward(femasr_net* net, const float* x_nchw, float* y_nchw, int
                         size_t workspace_bytes, void* stream);
 /* Algorithmic FLOPs (2*MAC; conv0 at K = 27) of one femasr_disc_forward, from a sizing run; 0 for a rejected geometry. */
 double femasr_disc_flops(femasr_net* net, int B, int H, int W);
+
+/* ------------------------------------------------------------------------------------------------
+ * LPIPS v0.1 (the lpips package's LPIPS(net='alex'|'vgg', lpips=True, spatial=False); pyiqa's metrics 'lpips' and
+ * 'lpips-vgg', which the training configs use for validation and as the perceptual loss), forward only:
+ *   x = (normalize ? 2x - 1 : x);  x = (x - shift) / scale;
+ *   f_k = the five ReLU taps of torchvision's alexnet().features (relu1 .. relu5) or vgg16().features (relu1_2 .. relu5_3);
+ *   r_k = mean_{h,w} sum_c w_k[c] (f0/(|f0|+1e-10) - f1/(|f1|+1e-10))^2;   d = r_0 + r_1 + r_2 + r_3 + r_4.
+ * The handle is a femasr_net: femasr_net_set_param / params_complete / set_profile / profile_json / last_launch_count /
+ * destroy work on it; the generator and discriminator entry points return FEMASR_ERR_ARG on it (their flops return 0),
+ * and the femasr_lpips_* ones on the other two kinds of handle.
+ * Parameters (the lpips package's state_dict names): scaling_layer.{shift,scale} [1,3,1,1];
+ * net.slice{1..5}.{i}.{weight,bias} with i the torchvision features index (alex: 0 | 3 | 6 | 8 | 10; vgg: 0,2 | 5,7 |
+ * 10,12,14 | 17,19,21 | 24,26,28); lin{0..4}.model.1.weight [1,C_k,1,1].
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int net;              /* 0 = alex, 1 = vgg (VGG16) */
+  int gemm_path;        /* 0 = fp32 SIMT implicit GEMM, 1 = wgmma split-fp16 tensor-core GEMM (no F8) */
+} femasr_lpips_config;
+int femasr_lpips_create(const femasr_lpips_config* cfg, femasr_net** out);
+/* Bytes of device workspace femasr_lpips_forward needs for a pair of [B,3,H,W] inputs.  vgg: H, W multiples of 16 (every
+ * pool exact); alex: H, W >= 31 (the smallest input torchvision's AlexNet features accept); else FEMASR_ERR_ARG. */
+int femasr_lpips_workspace_bytes(femasr_net* net, int B, int H, int W, size_t* bytes);
+/* x0, x1 [B,3,H,W] fp32 device -> dist [B] fp32 device (the lpips package's [B,1,1,1]) and, when per_layer is not NULL,
+ * per_layer [5][B] = r_k (retPerLayer).  normalize: inputs in [0,1] (pyiqa passes them so).  The backbone runs once over
+ * the 2B images; every r_k is a per-image mean accumulated in fp64 in a fixed order, so d(x, x) == 0 and
+ * d(x0, x1) == d(x1, x0) bit for bit. */
+int femasr_lpips_forward(femasr_net* net, const float* x0, const float* x1, float* dist, float* per_layer, int B, int H,
+                         int W, int normalize, void* workspace, size_t workspace_bytes, void* stream);
+/* Algorithmic FLOPs (2*MAC of the backbone convs; alex conv1 at K = 363, vgg conv1_1 at K = 27) of one
+ * femasr_lpips_forward (both images of every pair), from a sizing run; 0 for a rejected geometry. */
+double femasr_lpips_flops(femasr_net* net, int B, int H, int W);
+/* The LPIPS head of one tap: feat [2B,HW,C] fp32 NHWC (images of x0, then of x1), C a multiple of 64, w [C] the lin
+ * weights.  r[k*B + b] = mean over the HW pixels of sum_c w[c] (n0 - n1)^2 with n = f / (sqrt(sum_c f^2) + 1e-10), in
+ * one kernel: per-pixel values in fp32, their mean accumulated in fp64 in a fixed order and rounded once.  dist (may be
+ * NULL): also dist[b] = r[0*B+b] + ... + r[k*B+b], summed left to right.  scratch: femasr_lpips_head_scratch_bytes. */
+size_t femasr_lpips_head_scratch_bytes(int B, int HW);
+int femasr_lpips_head(const float* feat, const float* w, int B, int HW, int C, float* r, int k, float* dist,
+                      void* scratch, void* stream);
 
 /* layout helpers for tests */
 int femasr_nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, void* stream);
