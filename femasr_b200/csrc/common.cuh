@@ -155,4 +155,38 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   return v;
 }
 
+// The tail of a per-image fixed-order reduction over a grid (nblk, B) of NT-thread blocks (NT a power of two).  Every
+// thread of the block calls it; thread 0 passes the block's sum in `block_sum`, which is stored in
+// partial[b * nblk + blk].  The block that arrives last for image b sums that image's partials (thread-strided in index
+// order, then a tree over `red`, NT doubles of shared memory), resets count[b] for the next launch and returns true,
+// with the total in thread 0's `total`; every other block returns false.  The result depends only on the partials, not
+// on the block schedule or on the other images of the batch.
+template <int NT>
+__device__ __forceinline__ bool image_sum_last_block(double block_sum, double* __restrict__ partial,
+                                                     unsigned int* __restrict__ count, double* red, double& total) {
+  __shared__ bool last;
+  const int b = blockIdx.y, nblk = gridDim.x;
+  if (threadIdx.x == 0) {
+    partial[(long)b * nblk + blockIdx.x] = block_sum;
+    __threadfence();
+    last = atomicAdd(count + b, 1u) == (unsigned)(nblk - 1);
+  }
+  __syncthreads();
+  if (!last) return false;
+  __threadfence();
+  double t = 0.0;
+  for (int i = threadIdx.x; i < nblk; i += NT) t += __ldcg(partial + (long)b * nblk + i);
+  red[threadIdx.x] = t;
+  __syncthreads();
+  for (int o = NT / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    total = red[0];
+    count[b] = 0u;
+  }
+  return true;
+}
+
 }  // namespace femasr

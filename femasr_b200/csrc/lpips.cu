@@ -17,8 +17,7 @@ __global__ void __launch_bounds__(256) lpips_head_kernel(const float* __restrict
                                                          float* __restrict__ dist, double* __restrict__ partial,
                                                          unsigned int* __restrict__ count) {
   __shared__ double red[256];
-  __shared__ bool last;
-  const int b = blockIdx.y, nblk = gridDim.x;
+  const int b = blockIdx.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c2 = C / 2;
   const float2* w2 = reinterpret_cast<const float2*>(w);
@@ -49,33 +48,18 @@ __global__ void __launch_bounds__(256) lpips_head_kernel(const float* __restrict
   }
   if (lane == 0) red[warp] = acc;
   __syncthreads();
+  double blk = 0.0, total = 0.0;
+  if (threadIdx.x == 0)
+    for (int i = 0; i < HEAD_WARPS; ++i) blk += red[i];
+  if (!image_sum_last_block<256>(blk, partial, count, red, total)) return;
   if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int i = 0; i < HEAD_WARPS; ++i) t += red[i];
-    partial[(long)b * nblk + blockIdx.x] = t;
-    __threadfence();
-    last = atomicAdd(count + b, 1u) == (unsigned)(nblk - 1);
-  }
-  __syncthreads();
-  if (!last) return;
-  __threadfence();
-  double t = 0.0;
-  for (int i = threadIdx.x; i < nblk; i += 256) t += __ldcg(partial + (long)b * nblk + i);
-  red[threadIdx.x] = t;
-  __syncthreads();
-  for (int o = 128; o > 0; o >>= 1) {
-    if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    const float rk = (float)(red[0] / (double)HW);
+    const float rk = (float)(total / (double)HW);
     r[(long)k * B + b] = rk;
     if (dist) {
       float d = k == 0 ? rk : __ldcg(r + b);
       for (int j = 1; j <= k; ++j) d = __fadd_rn(d, j == k ? rk : __ldcg(r + (long)j * B + b));
       dist[b] = d;
     }
-    count[b] = 0u;
   }
 }
 

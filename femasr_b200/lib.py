@@ -14,6 +14,8 @@ LIB_PATH = os.environ.get("FEMASR_LIB") or os.path.join(_HERE, "libfemasr_b200.s
 PRO_NONE, PRO_GN_SILU, PRO_LN, PRO_GN_SILU_FAST, PRO_MAXPOOL2, PRO_BILINEAR2, PRO_MAXPOOL3S2 = 0, 1, 2, 3, 4, 5, 6
 ABI_VERSION = 4          # femasr_abi_version() of the library this binding was written against (include/femasr_b200.h)
 ACT_NONE, ACT_GELU, ACT_RELU, ACT_LRELU = 0, 1, 2, 3
+METRIC_PSNR, METRIC_SSIM = 0, 1
+METRIC_RGB, METRIC_Y_YIQ, METRIC_Y_YCBCR = 0, 1, 2
 TAP_STAGES = ("in_conv", "down", "swin", "up1", "up2", "z", "zq", "after_quant", "dec0", "dec1", "dec2")
 SEMANTIC_TAP_STAGES = ("vgg", "semantic")      # only in a forward that computes the semantic loss
 
@@ -150,6 +152,9 @@ SIGNATURES = {
     "femasr_lpips_flops": (_D, [_V, _I, _I, _I]),
     "femasr_lpips_head_scratch_bytes": (_Z, [_I, _I]),
     "femasr_lpips_head": (_I, [_V, _V, _I, _I, _I, _V, _I, _V, _V, _V]),
+    "femasr_metric_scratch_bytes": (_Z, [_I, _I, _I, _I, _I]),
+    "femasr_psnr": (_I, [_V, _V, _I, _I, _I, _I, _I, _V, _V, _V]),
+    "femasr_ssim": (_I, [_V, _V, _I, _I, _I, _I, _I, _V, _V, _V]),
 }
 
 _lib = None

@@ -468,6 +468,35 @@ size_t femasr_lpips_head_scratch_bytes(int B, int HW);
 int femasr_lpips_head(const float* feat, const float* w, int B, int HW, int C, float* r, int k, float* dist,
                       void* scratch, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * PSNR and SSIM as pyiqa's metrics `psnr` and `ssim` define them, the training configs' other two validation metrics.
+ * The definitions are recalled, not verified against pyiqa offline.  x, y [B,3,H,W] fp32 NCHW device, in [0, 1], not
+ * clamped; out [B] fp32 device, one score per image; scratch: femasr_metric_scratch_bytes.
+ *   mode FEMASR_METRIC_RGB: the three channels.  Otherwise the Y channel (pyiqa's test_y_channel=True), per pixel in
+ *   fp32 without contraction: Y_YIQ (color_space 'yiq', pyiqa's default) ((0.299 R + 0.587 G) + 0.114 B); Y_YCBCR
+ *   (color_space 'ycbcr', MATLAB's rgb2ycbcr) (((65.481 R + 128.553 G) + 24.966 B) + 16) / 255.
+ *   crop: crop_border pixels removed from every side.
+ * PSNR: at data range 1, mse = mean over channels and pixels of (x - y)^2 (difference in fp32, squares summed in fp64),
+ *   score = 10 log10(1 / (mse + 1e-8)) rounded to fp32 once (80 for identical images).
+ * SSIM (Wang et al.): at data range 255 (Y: round half to even of Y * 255, as pyiqa's to_y_channel(x, 255); RGB: x * 255
+ *   unrounded), the normalised 11x11 Gaussian window of sigma 1.5 with 'valid' filtering (output (Hc-10) x (Wc-10)),
+ *   C1 = (0.01 * 255)^2, C2 = (0.03 * 255)^2, cs = relu((2 s_xy + C2) / (s_x^2 + s_y^2 + C2)),
+ *   map = (2 mu_x mu_y + C1) / (mu_x^2 + mu_y^2 + C1) * cs; score = the mean of the map over channels and pixels.
+ *   Moments and map in fp64.  downsample is not supported.
+ * Properties: psnr(x, x) == 80 and ssim(x, x) == 1 exactly; metric(x, y) == metric(y, x) bit for bit; an image's score
+ * does not depend on the other images of the batch.  Refused with FEMASR_ERR_ARG: a null pointer, B outside [1, 65535],
+ * crop < 0 or 2 crop >= H or W, SSIM on a cropped side below 11, an unknown mode.
+ * ---------------------------------------------------------------------------------------------- */
+enum { FEMASR_METRIC_PSNR = 0, FEMASR_METRIC_SSIM = 1 };
+enum { FEMASR_METRIC_RGB = 0, FEMASR_METRIC_Y_YIQ = 1, FEMASR_METRIC_Y_YCBCR = 2 };
+/* Scratch bytes of one femasr_psnr (kind FEMASR_METRIC_PSNR) or femasr_ssim (FEMASR_METRIC_SSIM) call; 0 for arguments
+ * the call would refuse. */
+size_t femasr_metric_scratch_bytes(int kind, int B, int H, int W, int crop);
+int femasr_psnr(const float* x, const float* y, int B, int H, int W, int crop, int mode, float* out, void* scratch,
+                void* stream);
+int femasr_ssim(const float* x, const float* y, int B, int H, int W, int crop, int mode, float* out, void* scratch,
+                void* stream);
+
 /* layout helpers for tests */
 int femasr_nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, void* stream);
 int femasr_nhwc_to_nchw(const float* x, float* y, int B, int C, int H, int W, void* stream);

@@ -10,23 +10,17 @@ alexnet / vgg16 checkpoint and an lpips lin-weights file.  GT images pair with L
 images are super-resolved and scored as one batch (FeMaSRNet.sr_uint8: identical per image to tensor2img(test(x))).
 Prints one line per image and the mean."""
 import argparse
-import glob
 import os
 import sys
 import warnings
 
-import cv2
 import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from basicsr.archs.femasr_arch import FeMaSRNet  # noqa: E402
+from femasr_b200.folders import paired_batches, rgb01  # noqa: E402
 from femasr_b200.lpips import LPIPS  # noqa: E402
-
-
-def rgb01(bgr_u8: torch.Tensor) -> torch.Tensor:
-    """uint8 BGR [B,h,w,3] -> fp32 RGB [B,3,h,w] / 255 (img2tensor(img) / 255)."""
-    return bgr_u8.flip(-1).permute(0, 3, 1, 2).float() / 255.0
 
 
 def main(argv=None):
@@ -53,26 +47,15 @@ def main(argv=None):
         metric = LPIPS(a.lpips, backbone_path=a.lpips_weights[0], lin_path=a.lpips_weights[1])
     metric = metric.to(dev)
 
-    groups = {}
-    for path in sorted(glob.glob(os.path.join(a.lq, "*"))):
-        img = cv2.imread(path, cv2.IMREAD_COLOR)
-        if img is None:
-            continue
-        gt = cv2.imread(os.path.join(a.gt, os.path.basename(path)), cv2.IMREAD_COLOR)
-        if gt is None or gt.shape[:2] != (img.shape[0] * a.scale, img.shape[1] * a.scale):
-            raise SystemExit(f"{path}: no ground truth of {a.scale}x its size under {a.gt}")
-        groups.setdefault(img.shape[:2], []).append((os.path.basename(path), img, gt))
     scores = {}
     with torch.no_grad():
-        for items in groups.values():
-            for i in range(0, len(items), a.batch):
-                chunk = items[i:i + a.batch]
-                lq = torch.from_numpy(np.stack([im for _, im, _ in chunk])).to(dev)
-                sr = net.sr_uint8(lq)
-                gt = torch.from_numpy(np.stack([g for _, _, g in chunk])).to(dev)
-                d = metric(rgb01(sr), rgb01(gt), normalize=True).view(-1).cpu()
-                for (name, _, _), v in zip(chunk, d.tolist()):
-                    scores[name] = v
+        for chunk in paired_batches(a.lq, a.gt, a.scale, a.batch):
+            lq = torch.from_numpy(np.stack([im for _, im, _ in chunk])).to(dev)
+            sr = net.sr_uint8(lq)
+            gt = torch.from_numpy(np.stack([g for _, _, g in chunk])).to(dev)
+            d = metric(rgb01(sr), rgb01(gt), normalize=True).view(-1).cpu()
+            for (name, _, _), v in zip(chunk, d.tolist()):
+                scores[name] = v
     for name in sorted(scores):
         print(f"{name} {scores[name]:.6f}")
     print(f"mean lpips ({a.lpips}) over {len(scores)} images: {np.mean(list(scores.values())):.6f}")
