@@ -246,59 +246,16 @@ extern "C" int femasr_in_conv4x4_split(const float* x, const float* w, const flo
   return in_conv_launch(x, w, bias, nullptr, y_hi, y_lo, B, Cin, H, W, Cout, stream);
 }
 
-// in_conv on the tensor cores: the 4x4x3 patch of every output pixel as one K = 48 (padded to 64) row of split-fp16
-// operand planes, consumed by femasr_tc_igemm as a 1x1 "linear" (femasr_arch.py:150).  k = (kh * 4 + kw) * 3 + ci.
-__global__ void __launch_bounds__(256) in_conv_im2col_kernel(const float* __restrict__ x, uint4* __restrict__ hi,
-                                                             uint4* __restrict__ lo, int B, int H, int W, long total) {
-  const long i = (long)blockIdx.x * 256 + threadIdx.x;      // (output pixel, 8-wide k chunk)
-  if (i >= total) return;
-  const int j = (int)(i & 7);
-  const long m = i >> 3;
-  const int Ho = H - 1, Wo = W - 1;
-  const int ox = (int)(m % Wo);
-  const long t = m / Wo;
-  const int oy = (int)(t % Ho), b = (int)(t / Ho);
-  __align__(16) __half h[8], l[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const int k = j * 8 + e;
-    float v = 0.f;
-    if (k < 48) {
-      const int tap = k / 3, ci = k - tap * 3;
-      const int iy = oy + (tap >> 2) - 1, ix = ox + (tap & 3) - 1;
-      if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = __ldg(x + (((long)b * 3 + ci) * H + iy) * W + ix);
-    }
-    const float cl = fminf(fmaxf(v, -65504.f), 65504.f);
-    h[e] = __float2half_rn(cl);
-    l[e] = __float2half_rn(cl - __half2float(h[e]));
-  }
-  hi[i] = *reinterpret_cast<const uint4*>(h);
-  lo[i] = *reinterpret_cast<const uint4*>(l);
-}
-
-// OIHW [Cout,3,4,4] -> [Cout][64] fp32 in the im2col K order, zero padded (then femasr_tc_pack_weight(.., Cout, 64, 1, 1))
-__global__ void in_conv_weight_pad_kernel(const float* __restrict__ w, float* __restrict__ out, int Cout) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= Cout * 64) return;
-  const int co = i >> 6, k = i & 63;
-  float v = 0.f;
-  if (k < 48) { const int tap = k / 3, ci = k - tap * 3; v = w[((co * 3 + ci) * 4 + (tap >> 2)) * 4 + (tap & 3)]; }
-  out[i] = v;
-}
-
+// in_conv on the tensor cores (femasr_arch.py:150): the 4x4 pad 1 window of the untransformed image as the 3-channel
+// im2col of femasr_vgg_im2col_ex, K = 48 padded to 64, consumed by femasr_tc_igemm as a 1x1 "linear"
 extern "C" int femasr_in_conv_im2col(const float* x, void* a_hi, void* a_lo, int B, int Cin, int H, int W, void* stream) {
   FEMASR_CHECK_ARG(x && a_hi && a_lo && B > 0 && H > 1 && W > 1, "in_conv_im2col: bad argument");
   FEMASR_CHECK_ARG(Cin == 3, "in_conv_im2col: Cin must be 3");
-  const long total = (long)B * (H - 1) * (W - 1) * 8;
-  in_conv_im2col_kernel<<<(unsigned)cdiv(total, 256), 256, 0, as_stream(stream)>>>(
-      x, reinterpret_cast<uint4*>(a_hi), reinterpret_cast<uint4*>(a_lo), B, H, W, total);
-  return launch_status("in_conv_im2col_kernel");
+  return femasr_vgg_im2col_ex(x, nullptr, B, H, W, 4, 1, 1, 64, nullptr, nullptr, 0, a_hi, a_lo, nullptr, stream);
 }
 
 extern "C" int femasr_in_conv_pad_weight(const float* w_oihw, float* w_padded, int Cout, void* stream) {
-  FEMASR_CHECK_ARG(w_oihw && w_padded && Cout > 0, "in_conv_pad_weight: bad argument");
-  in_conv_weight_pad_kernel<<<(unsigned)cdiv((long)Cout * 64, 256), 256, 0, as_stream(stream)>>>(w_oihw, w_padded, Cout);
-  return launch_status("in_conv_weight_pad_kernel");
+  return femasr_vgg_pad_weight_ex(w_oihw, w_padded, Cout, 4, 64, stream);
 }
 
 template <int CO>

@@ -306,6 +306,13 @@ static void build_disc_spec(femasr_net* n) {
   add_conv(n, "conv9", F, 1, 3);                                 // femasr_out_conv3x3_n, Cout 1
 }
 
+// An activation in the form a GEMM reads it: fp32 NHWC f (the SIMT GEMM, or a tensor-core GEMM that stages it itself), or
+// split-fp16 planes hi/lo (the tensor-core GEMM).  Ctx::operand decides which for the net's gemm_path.
+struct Operand {
+  float* f = nullptr;
+  void *hi = nullptr, *lo = nullptr;
+};
+
 // ---------------------------------------------------------------------------------------------
 // One conv / linear layer of the graph.  H, W: the conv-input size (low-res when upsample).  The operand is fp32 x, or
 // split-fp16 planes a_hi/a_lo a producer already wrote (tensor-core GEMM only); the result is fp32 y, or split planes
@@ -330,6 +337,8 @@ struct ConvDesc {
   bool sn = false;                                 // a spectral-norm layer: the weight's forms live on w.weight_orig
   int macs = 0;                                    // algorithmic MACs per output element if not Cin*k*k (im2col GEMMs)
   std::string wname() const { return w + (sn ? ".weight_orig" : ".weight"); }
+  ConvDesc& in(const Operand& a) { x = a.f; a_hi = a.hi; a_lo = a.lo; return *this; }
+  ConvDesc& out(const Operand& o) { y = o.f; o_hi = o.hi; o_lo = o.lo; return *this; }
 };
 
 static ConvDesc geom(const std::string& w, int B, int H, int W, int Cin, int Cout, int k) {
@@ -504,6 +513,49 @@ struct Ctx {
     if (ahi) ar.release(ahi);
   }
 
+  // an operand of n values in the form this net's GEMMs read: split planes on gemm_path 1, fp32 on gemm_path 0
+  Operand operand(size_t n) {
+    Operand a;
+    if (net->cfg.gemm_path == 1) { a.hi = ar.alloc((n + 1) / 2); a.lo = ar.alloc((n + 1) / 2); }
+    else a.f = ar.alloc(n);
+    return a;
+  }
+  void release(const Operand& a) {
+    if (a.lo) ar.release(a.lo);
+    if (a.hi) ar.release(a.hi);
+    if (a.f) ar.release(a.f);
+  }
+
+  // the next conv's operand from fp32 NHWC src [B,H,W,C] through a 2x2/2 max-pool (FEMASR_PRO_MAXPOOL2), a 3x3/2 one
+  // (FEMASR_PRO_MAXPOOL3S2) or a bilinear x2 (FEMASR_PRO_BILINEAR2): fused into the split on gemm_path 1, the fp32 kernel
+  // of the same operation on gemm_path 0
+  Operand stage(const char* name, int mode, const float* src, int B, int H, int W, int C) {
+    const int ho = mode == FEMASR_PRO_BILINEAR2 ? 2 * H : mode == FEMASR_PRO_MAXPOOL2 ? H / 2 : (H - 3) / 2 + 1;
+    const int wo = mode == FEMASR_PRO_BILINEAR2 ? 2 * W : mode == FEMASR_PRO_MAXPOOL2 ? W / 2 : (W - 3) / 2 + 1;
+    const Operand a = operand((size_t)B * ho * wo * C);
+    run(name, 0.0, [&] {
+      if (!a.f) return femasr_tc_prepare(src, a.hi, a.lo, mode, nullptr, nullptr, nullptr, nullptr, B, H, W, C, 0, 0.f, st);
+      if (mode == FEMASR_PRO_MAXPOOL2) return femasr_maxpool2(src, a.f, B, H, W, C, st);
+      if (mode == FEMASR_PRO_MAXPOOL3S2) return femasr_maxpool3s2(src, a.f, B, H, W, C, st);
+      return femasr_bilinear_up2(src, a.f, B, H, W, C, st);
+    });
+    return a;
+  }
+
+  // The operand of a 3-channel first conv (ks x ks taps, stride, zero pad) as a 1x1 GEMM over im2col_k(ks)-wide rows of
+  // N images: those of x0, or N / 2 of x0 then N / 2 of x1 when x1 is given; optionally 2x - 1 and (x - mean) / std
+  // first (femasr_vgg_im2col_ex).  The size comes from N alone: x0 and x1 are NULL in a sizing run.
+  Operand im2col(const char* name, const float* x0, const float* x1, int N, int H, int W, int ks, int stride, int pad,
+                 const float* mean, const float* sd, int two_x_minus_1) {
+    const int kpad = im2col_k(ks), ho = (H + 2 * pad - ks) / stride + 1, wo = (W + 2 * pad - ks) / stride + 1;
+    const Operand a = operand((size_t)N * ho * wo * kpad);
+    run(name, 0.0, [&] {
+      return femasr_vgg_im2col_ex(x0, x1, x1 ? N / 2 : N, H, W, ks, stride, pad, kpad, mean, sd, two_x_minus_1, a.hi, a.lo,
+                                  a.f, st);
+    });
+    return a;
+  }
+
   // GroupNorm partial sums produced by a tensor-core conv epilogue (see femasr_tc_args.gn_partial)
   struct Stats { float* partial = nullptr; int rows = 0; };
   // for the conv d that will produce them (none on the SIMT path)
@@ -625,63 +677,45 @@ struct Ctx {
   // vgg_feat = relu4_4((x - mean) / std) (femasr_arch.py:318-320).  Runs before the encoder: relu4_4 is allocated first
   // and every full-resolution VGG buffer is released before the encoder's peak.
   void semantic_vgg(const float* x_nchw, int B, int H, int W) {
-    const bool tc = net->cfg.gemm_path == 1;
     vgg_feat = ar.alloc((size_t)B * (H / 8) * (W / 8) * 512);
-    float *ahi = nullptr, *alo = nullptr, *af = nullptr;   // conv1_1's operand: split planes (tc) or fp32
-    const size_t rows = (size_t)B * H * W;
-    if (tc) { ahi = ar.alloc(rows * 32); alo = ar.alloc(rows * 32); } else { af = ar.alloc(rows * 64); }
-    const float *mean = P("vgg_feat_extractor.mean"), *sd = P("vgg_feat_extractor.std");
-    run("vgg_im2col", 0.0, [&] { return femasr_vgg_im2col(x_nchw, mean, sd, ahi, alo, af, B, H, W, st); });
-    vgg_stack(VGG19_RELU4_4, 12, "vgg_feat_extractor.vgg_net.", "vgg_conv", "vgg_pool", B, H, W, ahi, alo, af, vgg_feat,
+    const Operand a = im2col("vgg_im2col", x_nchw, nullptr, B, H, W, 3, 1, 1, P("vgg_feat_extractor.mean"),
+                             P("vgg_feat_extractor.std"), 0);
+    vgg_stack(VGG19_RELU4_4, 12, "vgg_feat_extractor.vgg_net.", "vgg_conv", "vgg_pool", B, H, W, a, vgg_feat,
               [](const float*, int, int, int) {});
     tap("vgg", vgg_feat, (size_t)B * (H / 8) * (W / 8) * 512);
   }
 
-  // The convs of a VggLayer table over B images of H x W, from conv 0's im2col operand (K = 27 -> 64: split planes ahi/alo
-  // on gemm_path 1, fp32 rows af on gemm_path 0), which this releases.  gemm_path 1 hands the activations from conv to
-  // conv as split fp16 planes; the pools read fp32 (pooling before the split) and write the next conv's planes.  Every
-  // conv is bias + ReLU: the 3-product split-fp16 wgmma GEMM on gemm_path 1, the fp32 SIMT GEMM on gemm_path 0.
-  // on_tap(f, h, w, c) sees the fp32 output of every tap layer while it is alive.  The last conv writes into `last` if
-  // given, else into an arena buffer that is returned for the caller to release.
+  // The convs of a VggLayer table over B images of H x W, from conv 0's im2col operand a (K = 27 -> 64), which this
+  // releases.  A conv's output goes on as the next conv's operand; it is fp32 where the caller, a tap or a pool reads it
+  // (the pools stage the next operand from fp32).  Every conv is bias + ReLU: the 3-product split-fp16 wgmma GEMM on
+  // gemm_path 1, the fp32 SIMT GEMM on gemm_path 0.  on_tap(f, h, w, c) sees the fp32 output of every tap layer while it
+  // is alive.  The last conv writes into `last` if given, else into an arena buffer that is returned for the caller to
+  // release.
   template <class F>
   float* vgg_stack(const VggLayer* L, int nl, const std::string& pre, const char* conv_name, const char* pool_name, int B,
-                   int H, int W, float* ahi, float* alo, float* af, float* last, F&& on_tap) {
-    const bool tc = net->cfg.gemm_path == 1;
+                   int H, int W, Operand a, float* last, F&& on_tap) {
     int h = H, w = W, c = 64;
-    float* f = nullptr;                                    // fp32 output in front of a pool
-    float* y = nullptr;
+    float* y = nullptr;                                    // the previous conv's output, fp32 in front of a pool
     for (int i = 0; i < nl; ++i) {
       const int co = L[i].cout;
       if (L[i].pool_before) {
-        const size_t n2 = (size_t)B * (h / 2) * (w / 2) * c;
-        if (tc) {
-          ahi = ar.alloc((n2 + 1) / 2); alo = ar.alloc((n2 + 1) / 2);
-          const int hh = h, ww = w, cc = c;
-          run(pool_name, 0.0, [&] {
-            return femasr_tc_prepare(f, ahi, alo, FEMASR_PRO_MAXPOOL2, nullptr, nullptr, nullptr, nullptr, B, hh, ww, cc, 0, 0.f, st);
-          });
-        } else {
-          af = ar.alloc(n2);
-          const int hh = h, ww = w, cc = c;
-          run(pool_name, 0.0, [&] { return femasr_maxpool2(f, af, B, hh, ww, cc, st); });
-        }
-        ar.release(f); f = nullptr;
+        a = stage(pool_name, FEMASR_PRO_MAXPOOL2, y, B, h, w, c);
+        ar.release(y);
         h /= 2; w /= 2;
       }
-      const bool lastl = i == nl - 1, to_f32 = !tc || lastl || L[i].tap || L[i + 1].pool_before;
+      const bool lastl = i == nl - 1;
       const size_t n = (size_t)B * h * w * co;
-      y = lastl && last ? last : (to_f32 ? ar.alloc(n) : nullptr);
-      float *ohi = nullptr, *olo = nullptr;
-      if (!to_f32) { ohi = ar.alloc((n + 1) / 2); olo = ar.alloc((n + 1) / 2); }
+      Operand o;
+      if (lastl && last) o.f = last;
+      else if (lastl || L[i].tap || L[i + 1].pool_before) o.f = ar.alloc(n);
+      else o = operand(n);
       // conv 0: 1x1 GEMM over the K = 27 -> 64 im2col rows (27 algorithmic MACs)
       ConvDesc g = geom(pre + L[i].w, B, h, w, i == 0 ? 64 : c, co, i == 0 ? 1 : 3);
       g.name = conv_name; g.semantic = true; g.im2col = i == 0; g.macs = i == 0 ? 27 : 0; g.act = FEMASR_ACT_RELU;
-      g.x = af; g.a_hi = ahi; g.a_lo = alo; g.y = y; g.o_hi = ohi; g.o_lo = olo;
-      conv(g);
-      if (tc) { ar.release(alo); ar.release(ahi); ahi = ohi; alo = olo; }
-      else { ar.release(af); af = y; }
+      conv(g.in(a).out(o));
+      release(a);
+      a = o; y = o.f;
       if (L[i].tap) on_tap(y, h, w, co);
-      if (to_f32 && !lastl) f = y;
       c = co;
     }
     return y;
@@ -692,7 +726,7 @@ struct Ctx {
   // it is alive and is released as soon as the next layer has read it.  r [5][B] is per_layer, or workspace.  Numerics
   // are those of the semantic loss's VGG convs: the 3-product split-fp16 GEMM without F8 on gemm_path 1, fp32 SIMT on 0.
   void lpips(const float* x0, const float* x1, float* dist, float* per_layer, int B, int H, int W, int normalize) {
-    const bool tc = net->cfg.gemm_path == 1, vgg = net->lcfg.net == 1;
+    const bool vgg = net->lcfg.net == 1;
     const int N = 2 * B;
     float* r = per_layer ? per_layer : ar.alloc((size_t)5 * B);
     int tap_k = 0;
@@ -705,57 +739,35 @@ struct Ctx {
       ++tap_k;
     };
     // first conv's operand: im2col of the scaled pair (vgg: 3x3 pad 1, K = 27 -> 64; alex: 11x11 stride 4 pad 2, K = 363 -> 384)
-    const int ks = vgg ? 3 : 11, stride = vgg ? 1 : 4, pad = vgg ? 1 : 2, kpad = im2col_k(ks);
-    const int h1 = (H + 2 * pad - ks) / stride + 1, w1 = (W + 2 * pad - ks) / stride + 1;
-    const size_t rows = (size_t)N * h1 * w1;
-    float *ahi = nullptr, *alo = nullptr, *af = nullptr;
-    if (tc) { ahi = ar.alloc(rows * kpad / 2); alo = ar.alloc(rows * kpad / 2); } else { af = ar.alloc(rows * kpad); }
-    const float *shift = P("scaling_layer.shift"), *scale = P("scaling_layer.scale");
-    run("lpips_im2col", 0.0, [&] {
-      return femasr_vgg_im2col_ex(x0, x1, B, H, W, ks, stride, pad, kpad, shift, scale, normalize, ahi, alo, af, st);
-    });
-    if (vgg) ar.release(vgg_stack(VGG16_LPIPS, 13, "", "lpips_conv", "lpips_pool", N, H, W, ahi, alo, af, nullptr, head));
-    else alex(ahi, alo, af, N, h1, w1, head);
+    const int ks = vgg ? 3 : 11, stride = vgg ? 1 : 4, pad = vgg ? 1 : 2;
+    const Operand a = im2col("lpips_im2col", x0, x1, N, H, W, ks, stride, pad, P("scaling_layer.shift"),
+                             P("scaling_layer.scale"), normalize);
+    if (vgg) ar.release(vgg_stack(VGG16_LPIPS, 13, "", "lpips_conv", "lpips_pool", N, H, W, a, nullptr, head));
+    else alex(a, N, (H + 2 * pad - ks) / stride + 1, (W + 2 * pad - ks) / stride + 1, head);
     if (!per_layer) ar.release(r);
   }
 
-  // AlexNet features (torchvision): conv1 (the im2col GEMM) | pool 3/2, conv2 5x5 pad 2 | pool 3/2, conv3 | conv4 | conv5,
-  // each conv + ReLU and each ReLU a tap.  h, w: conv1's output size.  Releases conv1's operand.
+  // AlexNet features (torchvision): conv1 (the im2col GEMM over a) | pool 3/2, conv2 5x5 pad 2 | pool 3/2, conv3 | conv4 |
+  // conv5, each conv + ReLU and each ReLU a tap.  h, w: conv1's output size.  Releases conv1's operand.
   template <class F>
-  void alex(float* ahi, float* alo, float* af, int N, int h, int w, F&& head) {
-    const bool tc = net->cfg.gemm_path == 1;
+  void alex(Operand a, int N, int h, int w, F&& head) {
     float* f = nullptr;                                    // the previous conv's fp32 output
     for (int i = 0; i < 5; ++i) {
       const AlexLayer& l = ALEX_LPIPS[i];
-      float *phi = nullptr, *plo = nullptr, *pf = nullptr;  // max-pool 3/2 output in front of conv2 and conv3
-      if (i == 1 || i == 2) {
-        const int hp = (h - 3) / 2 + 1, wp = (w - 3) / 2 + 1, hh = h, ww = w, cc = l.cin;
-        const size_t n2 = (size_t)N * hp * wp * l.cin;
-        const float* src = f;
-        if (tc) {
-          phi = ar.alloc((n2 + 1) / 2); plo = ar.alloc((n2 + 1) / 2);
-          run("lpips_pool", 0.0, [&] {
-            return femasr_tc_prepare(src, phi, plo, FEMASR_PRO_MAXPOOL3S2, nullptr, nullptr, nullptr, nullptr, N, hh, ww, cc, 0, 0.f, st);
-          });
-        } else {
-          pf = ar.alloc(n2);
-          run("lpips_pool", 0.0, [&] { return femasr_maxpool3s2(src, pf, N, hh, ww, cc, st); });
-        }
-        ar.release(f); f = nullptr;
-        h = hp; w = wp;
+      if (i == 1 || i == 2) {                              // max-pool 3/2 in front of conv2 and conv3
+        a = stage("lpips_pool", FEMASR_PRO_MAXPOOL3S2, f, N, h, w, l.cin);
+        ar.release(f);
+        h = (h - 3) / 2 + 1; w = (w - 3) / 2 + 1;
+      } else if (i > 0) {
+        a = Operand{f};
       }
       float* y = ar.alloc((size_t)N * h * w * l.cout);
       // conv1: 1x1 GEMM over the K = 363 -> 384 im2col rows (363 algorithmic MACs)
       ConvDesc g = geom(l.w, N, h, w, i == 0 ? im2col_k(l.k) : l.cin, l.cout, i == 0 ? 1 : l.k);
       g.name = "lpips_conv"; g.semantic = true; g.act = FEMASR_ACT_RELU; g.y = y;
-      if (i == 0) { g.im2col = true; g.macs = 3 * l.k * l.k; g.x = af; g.a_hi = ahi; g.a_lo = alo; }
-      else if (phi) { g.a_hi = phi; g.a_lo = plo; }
-      else { g.x = pf ? pf : f; }
-      conv(g);
-      if (i == 0) { if (tc) { ar.release(alo); ar.release(ahi); } else { ar.release(af); } }
-      if (phi) { ar.release(plo); ar.release(phi); }
-      if (pf) ar.release(pf);
-      if (f) ar.release(f);
+      if (i == 0) { g.im2col = true; g.macs = 3 * l.k * l.k; }
+      conv(g.in(a));
+      release(a);
       f = y;
       head(f, h, w, l.cout);
     }
@@ -767,22 +779,15 @@ struct Ctx {
   // stage, so the sum over levels (:372) is this one term.
   void semantic_loss(const float* zq, int B, int hh, int ww) {
     const size_t N = (size_t)B * hh * ww;
-    const bool tc = net->cfg.gemm_path == 1;
     float* s = ar.alloc(N * 512);
     float* rows = ar.alloc(N);
-    float *zhi = nullptr, *zlo = nullptr;
-    if (tc) {
-      zhi = ar.alloc(N * 256); zlo = ar.alloc(N * 256);
-      run("tc_prepare", 0.0, [&] { return femasr_tc_prepare(zq, zhi, zlo, FEMASR_PRO_NONE, nullptr, nullptr, nullptr, nullptr, B, hh, ww, 512, 0, 0.f, st); });
-    }
     ConvDesc g = geom("conv_semantic.0", B, hh, ww, 512, 512, 1);
-    g.name = "semantic_conv"; g.semantic = true; g.act = FEMASR_ACT_RELU; g.x = zq; g.a_hi = zhi; g.a_lo = zlo; g.y = s;
+    g.name = "semantic_conv"; g.semantic = true; g.act = FEMASR_ACT_RELU; g.x = zq; g.y = s;
     conv(g);
     tap("semantic", s, N * 512);
     const float* v = vgg_feat;
     run("semantic_mse", 0.0, [&] { return femasr_sq_diff_rows(s, v, rows, (int)N, 512, st); });
     run("semantic_mse", 0.0, [&] { return femasr_sum_scaled(rows, sem_loss, N, 1.0 / ((double)N * 512), st); });
-    if (tc) { ar.release(zlo); ar.release(zhi); }
     ar.release(rows); ar.release(s);
     ar.release(vgg_feat); vgg_feat = nullptr;
   }
@@ -936,7 +941,7 @@ struct Ctx {
     precise_region = true;
     const float *iw = P(enc + ".in_conv.weight"), *ib = P(enc + ".in_conv.bias");
     float* cur = nullptr;                 // fp32 in_conv output (SIMT path, or when its tap is requested)
-    float* in_hi = nullptr; float* in_lo = nullptr;   // tensor-core path: in_conv writes the split operand planes directly
+    Operand in_split;                     // tensor-core path: in_conv writes the down conv's split operand planes directly
     const size_t in_elems = (size_t)B * h * w * c;
     if (!tc || tapped("in_conv")) {       // identical in the sizing run and the real run: taps are registered first
       cur = ar.alloc(in_elems);
@@ -946,18 +951,13 @@ struct Ctx {
       tap("in_conv", cur, in_elems);
     }
     if (tc) {
-      // K = 48 (-> 64) GEMM over im2col rows on the tensor cores, writing the down conv's split planes
-      in_hi = ar.alloc((in_elems + 1) / 2);
-      in_lo = ar.alloc((in_elems + 1) / 2);
-      const size_t rows = (size_t)B * h * w;
-      float* ic_hi = ar.alloc(rows * 64 / 2);
-      float* ic_lo = ar.alloc(rows * 64 / 2);
-      run("in_conv_im2col", 0.0, [&] { return femasr_in_conv_im2col(x_nchw, ic_hi, ic_lo, B, cfg.in_channel, H, W, st); });
+      // K = 48 (-> 64) GEMM over im2col rows on the tensor cores
+      in_split = operand(in_elems);
+      const Operand a = im2col("in_conv_im2col", x_nchw, nullptr, B, H, W, 4, 1, 1, nullptr, nullptr, 0);
       ConvDesc g = geom(enc + ".in_conv", B, h, w, 64, c, 1);
       g.name = "in_conv"; g.im2col = true; g.macs = 16 * cfg.in_channel;
-      g.a_hi = ic_hi; g.a_lo = ic_lo; g.o_hi = in_hi; g.o_lo = in_lo;
-      conv(g);
-      ar.release(ic_lo); ar.release(ic_hi);
+      conv(g.in(a).out(in_split));
+      release(a);
     }
     // which enc_feats the decoder loop reads: at quantising levels (before_quant input) and, in the LQ stage with
     // use_residual, at the other levels > 0 (skip adds)
@@ -971,11 +971,11 @@ struct Ctx {
       float* nxt = ar.alloc((size_t)B * ho * wo * co);
       ConvDesc g = geom(b + ".0", B, h, w, c, co, 3);
       g.stride = 2; g.x = cur; g.y = nxt;
-      if (i == 0) { g.a_hi = in_hi; g.a_lo = in_lo; }
+      if (i == 0) { g.a_hi = in_split.hi; g.a_lo = in_split.lo; }
       const Stats sd0 = alloc_stats(g);
       g.gn_partial = sd0.partial;
       conv(g);
-      if (i == 0 && in_lo) { ar.release(in_lo); ar.release(in_hi); in_lo = in_hi = nullptr; }
+      if (i == 0) release(in_split);
       // HQ stage: enc_feats = the down blocks' outputs reversed (:316); block i-1's output is level d-i
       if (cur) { if (net->hq && i > 0 && need[d - i]) feats[d - i] = cur; else ar.release(cur); }
       cur = nxt; h = ho; w = wo; c = co;
@@ -1028,17 +1028,13 @@ struct Ctx {
       g.name = "disc_conv"; g.sn = true; g.bias = false; g.act = FEMASR_ACT_LRELU;
       return g;
     };
-    {  // conv0: 3x3 pad 1, 3 -> F, as a 1x1 GEMM over femasr_vgg_im2col's unnormalised K = 27 (-> 64) rows
-      const size_t rows = (size_t)B * H * W;
-      xs[0] = ar.alloc(rows * F);
-      float *ahi = nullptr, *alo = nullptr, *af = nullptr;
-      if (tc) { ahi = ar.alloc(rows * 32); alo = ar.alloc(rows * 32); } else { af = ar.alloc(rows * 64); }
-      run("disc_im2col", 0.0, [&] { return femasr_vgg_im2col(x_nchw, nullptr, nullptr, ahi, alo, af, B, H, W, st); });
+    {  // conv0: 3x3 pad 1, 3 -> F, as a 1x1 GEMM over unnormalised K = 27 (-> 64) im2col rows
+      xs[0] = ar.alloc((size_t)B * H * W * F);
+      const Operand a = im2col("disc_im2col", x_nchw, nullptr, B, H, W, 3, 1, 1, nullptr, nullptr, 0);
       ConvDesc g = geom("conv0", B, H, W, 64, F, 1);
-      g.name = "disc_conv"; g.im2col = true; g.macs = 27; g.act = FEMASR_ACT_LRELU;
-      g.x = af; g.a_hi = ahi; g.a_lo = alo; g.y = xs[0];
-      conv(g);
-      if (tc) { ar.release(alo); ar.release(ahi); } else { ar.release(af); }
+      g.name = "disc_conv"; g.im2col = true; g.macs = 27; g.act = FEMASR_ACT_LRELU; g.y = xs[0];
+      conv(g.in(a));
+      release(a);
     }
     for (int i = 1; i <= 3; ++i) {   // conv1 .. conv3: 4x4 stride 2 pad 1
       xs[i] = ar.alloc((size_t)B * hs[i] * ws[i] * (F << i));
@@ -1047,61 +1043,28 @@ struct Ctx {
       conv(g);
     }
     // conv4 .. conv6: 3x3 on bilinear_x2 of the previous output, then + x2 / x1 / x0
-    float* cur = xs[3];
-    void *p_hi = nullptr, *p_lo = nullptr;                 // conv6's output as split planes (tensor-core path)
+    Operand o{xs[3]};                                      // the previous conv's output (fp32 in front of an upsample)
     for (int lv = 2; lv >= 0; --lv) {
-      const int ci = F << (lv + 1), co = F << lv, h = hs[lv], w = ws[lv], hl = hs[lv + 1], wl = ws[lv + 1];
-      const size_t n_in = (size_t)B * h * w * ci, n_out = (size_t)B * h * w * co;
+      const int ci = F << (lv + 1), co = F << lv, h = hs[lv], w = ws[lv];
       ConvDesc g = sn_conv(6 - lv, h, w, ci, co, 3);
       g.res1 = skip ? xs[lv] : nullptr;
-      float *uhi = nullptr, *ulo = nullptr, *uf = nullptr;
-      const float* src = cur;
-      if (tc) {
-        uhi = ar.alloc((n_in + 1) / 2); ulo = ar.alloc((n_in + 1) / 2);
-        run("disc_up", 0.0, [&] {
-          return femasr_tc_prepare(src, uhi, ulo, FEMASR_PRO_BILINEAR2, nullptr, nullptr, nullptr, nullptr, B, hl, wl, ci, 0, 0.f, st);
-        });
-        g.a_hi = uhi; g.a_lo = ulo;
-      } else {
-        uf = ar.alloc(n_in);
-        run("disc_up", 0.0, [&] { return femasr_bilinear_up2(src, uf, B, hl, wl, ci, st); });
-        g.x = uf;
-      }
-      ar.release(cur);
-      cur = nullptr;
-      if (lv == 0 && tc) {
-        p_hi = ar.alloc((n_out + 1) / 2); p_lo = ar.alloc((n_out + 1) / 2);
-        g.o_hi = p_hi; g.o_lo = p_lo;
-      } else {
-        cur = ar.alloc(n_out);
-        g.y = cur;
-      }
-      conv(g);
-      if (tc) { ar.release(ulo); ar.release(uhi); } else { ar.release(uf); }
+      const Operand u = stage("disc_up", FEMASR_PRO_BILINEAR2, o.f, B, hs[lv + 1], ws[lv + 1], ci);
+      ar.release(o.f);
+      const size_t n_out = (size_t)B * h * w * co;
+      o = lv == 0 ? operand(n_out) : Operand{ar.alloc(n_out)};
+      conv(g.in(u).out(o));
+      release(u);
       ar.release(xs[lv]);
     }
     // conv7, conv8 (3x3 F -> F), then conv9 (3x3 F -> 1, bias) on the out_conv kernels
     const size_t nf = (size_t)B * H * W * F;
     ConvDesc g7 = sn_conv(7, H, W, F, F, 3), g8 = sn_conv(8, H, W, F, F, 3);
     float* x8 = ar.alloc(nf);
-    if (tc) {
-      void* q_hi = ar.alloc((nf + 1) / 2);
-      void* q_lo = ar.alloc((nf + 1) / 2);
-      g7.a_hi = p_hi; g7.a_lo = p_lo; g7.o_hi = q_hi; g7.o_lo = q_lo;
-      conv(g7);
-      ar.release(p_lo); ar.release(p_hi);
-      g8.a_hi = q_hi; g8.a_lo = q_lo; g8.y = x8;
-      conv(g8);
-      ar.release(q_lo); ar.release(q_hi);
-    } else {
-      float* x7 = ar.alloc(nf);
-      g7.x = cur; g7.y = x7;
-      conv(g7);
-      ar.release(cur);
-      g8.x = x7; g8.y = x8;
-      conv(g8);
-      ar.release(x7);
-    }
+    const Operand q = operand(nf);
+    conv(g7.in(o).out(q));
+    release(o);
+    conv(g8.in(q).out(Operand{x8}));
+    release(q);
     const float *w9 = P("conv9.weight"), *b9 = P("conv9.bias");
     run("disc_head", 2.0 * 9 * F * (double)B * H * W,
         [&] { return femasr_out_conv3x3_n(x8, w9, b9, y_nchw, B, H, W, F, 1, tc ? 1 : 0, st); });
@@ -1180,7 +1143,7 @@ static int pack_forms(femasr_net* net, DevParam& d, const ParamInfo& pi, const f
     const int kp = im2col_k(k);
     float* tmp = nullptr;
     FEMASR_CUDA(cudaMallocAsync(&tmp, (size_t)co * kp * sizeof(float), st));
-    s = k == 4 ? femasr_in_conv_pad_weight(src, tmp, co, st) : femasr_vgg_pad_weight_ex(src, tmp, co, k, kp, st);
+    s = femasr_vgg_pad_weight_ex(src, tmp, co, k, kp, st);
     if (!s) s = ensure(&d.im2col, tc ? femasr_tc_weight_bytes(co, kp, 1, 1) : (size_t)co * kp * sizeof(float));
     if (!s) s = tc ? femasr_tc_pack_weight(tmp, d.im2col, co, kp, 1, 1, st)
                    : femasr_pack_weight(tmp, static_cast<float*>(d.im2col), co, kp, 1, 1, st);

@@ -1,8 +1,8 @@
 // The small kernels of the HQ stage's semantic loss (femasr_arch.py:301-309, 318-320, 344-347): the normalising
-// im2col of VGG19's conv1_1 (also LPIPS' first conv and the discriminator's conv0), the fp32 max-pools of the SIMT path
-// and the squared-difference rows of the MSE.  The
-// twelve VGG convs and conv_semantic themselves run on femasr_tc_igemm / femasr_igemm_simt with the ReLU epilogue,
-// and the pool of the tensor-core path is femasr_tc_prepare's FEMASR_PRO_MAXPOOL2 mode.
+// im2col of VGG19's conv1_1 (also LPIPS' first conv, the discriminator's conv0 and the generator's tensor-core in_conv),
+// the fp32 max-pools of the SIMT path and the squared-difference rows of the MSE.  The twelve VGG convs and
+// conv_semantic themselves run on femasr_tc_igemm / femasr_igemm_simt with the ReLU epilogue, and the pool of the
+// tensor-core path is femasr_tc_prepare's FEMASR_PRO_MAXPOOL2 mode.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -12,14 +12,19 @@ namespace femasr {
 // The operand of a 3-channel first conv as a 1x1 GEMM: per output pixel the ks x ks window (stride, pad) of the
 // transformed image, k = (kh * ks + kw) * 3 + ci, zero padded to kpad (a multiple of 64).  Thread = (pixel, 8-wide k
 // chunk).  The transform is x' = 2x - 1 when two_x_minus_1 (LPIPS normalize=True), then (x' - mean) / std as a true
-// division (vgg_arch.py forward, LPIPS' ScalingLayer); mean == NULL: the window of x itself (the discriminator's conv0).
-// Images [0, B0) come from x0, the rest from x1 (the two inputs of a pair without a concatenated copy).
+// division (vgg_arch.py forward, LPIPS' ScalingLayer); mean == NULL: the window of x itself (the discriminator's conv0,
+// the generator's in_conv).
+// Images [0, B0) come from x0, the rest from x1 (the two inputs of a pair without a concatenated copy).  KS, KPAD: the
+// window and row width of one of the engine's first convs as constants (the index arithmetic is then shifts and
+// multiplies), or 0, 0 for both at run time.
+template <int KS, int KPAD>
 __global__ void __launch_bounds__(256) vgg_im2col_kernel(const float* __restrict__ x0, const float* __restrict__ x1,
                                                          int B0, const float* __restrict__ mean,
                                                          const float* __restrict__ stdv, int two_x_minus_1,
                                                          uint4* __restrict__ hi, uint4* __restrict__ lo,
-                                                         float4* __restrict__ f32, int H, int W, int Ho, int Wo, int ks,
-                                                         int stride, int pad, int kc8, long total) {
+                                                         float4* __restrict__ f32, int H, int W, int Ho, int Wo, int ks_rt,
+                                                         int stride, int pad, int kc8_rt, long total) {
+  const int ks = KS ? KS : ks_rt, kc8 = KPAD ? KPAD / 8 : kc8_rt;
   const long i = (long)blockIdx.x * 256 + threadIdx.x;
   if (i >= total) return;
   const int j = (int)(i % kc8);
@@ -114,7 +119,11 @@ extern "C" int femasr_vgg_im2col_ex(const float* x0, const float* x1, int B, int
   const int Ho = (H + 2 * pad - ksize) / stride + 1, Wo = (W + 2 * pad - ksize) / stride + 1;
   FEMASR_CHECK_ARG(H + 2 * pad >= ksize && W + 2 * pad >= ksize, "vgg_im2col: input smaller than the window");
   const long total = (long)(x1 ? 2 * B : B) * Ho * Wo * (kpad / 8);
-  vgg_im2col_kernel<<<(unsigned)cdiv(total, 256), 256, 0, as_stream(stream)>>>(
+  auto kernel = vgg_im2col_kernel<0, 0>;
+  if (ksize == 3 && kpad == 64) kernel = vgg_im2col_kernel<3, 64>;          // VGG conv1_1, the discriminator's conv0
+  if (ksize == 4 && kpad == 64) kernel = vgg_im2col_kernel<4, 64>;          // the generator's in_conv
+  if (ksize == 11 && kpad == 384) kernel = vgg_im2col_kernel<11, 384>;      // AlexNet's conv1
+  kernel<<<(unsigned)cdiv(total, 256), 256, 0, as_stream(stream)>>>(
       x0, x1, B, mean, std_, two_x_minus_1 ? 1 : 0, reinterpret_cast<uint4*>(a_hi), reinterpret_cast<uint4*>(a_lo),
       reinterpret_cast<float4*>(a_f32), H, W, Ho, Wo, ksize, stride, pad, kpad / 8, total);
   return launch_status("vgg_im2col_kernel");

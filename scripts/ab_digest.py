@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Digest of the public-surface outputs, the launch count and the per-kernel (launches, flops) profile of a set of cases on
-both GEMM paths, with the library selected by FEMASR_LIB: two library builds that claim to be arithmetic-identical (an
-epilogue / scheduling / host-graph refactor) must print the same JSON.
+"""Digest of the public-surface outputs, the launch count and the per-kernel (launches, flops) profile of a set of generator,
+discriminator and LPIPS cases on both GEMM paths, with the library selected by FEMASR_LIB: two library builds that claim to
+be arithmetic-identical (an epilogue / scheduling / host-graph refactor) must print the same JSON.
     FEMASR_LIB=... python scripts/ab_digest.py > a.json
 Runs eagerly (FEMASR_CUDA_GRAPH=0) so that every launch is counted and profiled."""
 import hashlib
@@ -15,9 +15,11 @@ os.environ.setdefault("FEMASR_CUDA_GRAPH", "0")
 import torch  # noqa: E402
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from basicsr.archs.discriminator_arch import UNetDiscriminatorSN  # noqa: E402
 from basicsr.archs.femasr_arch import FeMaSRNet  # noqa: E402
 from femasr_b200.lib import TAP_STAGES  # noqa: E402
-from femasr_b200.spec import random_state_dict  # noqa: E402
+from femasr_b200.lpips import LPIPS  # noqa: E402
+from femasr_b200.spec import random_disc_state_dict, random_lpips_state_dict, random_state_dict  # noqa: E402
 
 
 def dig(t):
@@ -52,6 +54,11 @@ def case(out, key, net, dev, fn):
 def fwd(net, x, gt=None):
     y, loss, sem, idx = net(x, gt_indices=gt)
     return [y, loss, sem, *idx]
+
+
+def lpips_fwd(net, x0, x1, normalize):
+    d, r = net(x0, x1, retPerLayer=True, normalize=normalize)
+    return [d, *r]
 
 
 def taps_fwd(eng, x):
@@ -93,6 +100,22 @@ def main():
             gt = [torch.randint(0, n_e, i.shape, generator=g).to(dev) for i, (_s, n_e, _e) in zip(net(x)[3], cb)]
             case(out, f"gp{gp}/x{scale}_cb{len(cb)}_fwd", net, dev, lambda: fwd(net, x))
             case(out, f"gp{gp}/x{scale}_cb{len(cb)}_fwd_gt", net, dev, lambda: fwd(net, x, gt))
+        x = rand((2, 3, 64, 96), 13).to(dev)
+        for skip in (0, 1):
+            net = UNetDiscriminatorSN(3, skip_connection=skip, gemm_path=gp)
+            net.load_state_dict(random_disc_state_dict(14), strict=True)
+            net = net.to(dev).eval()
+            case(out, f"gp{gp}/disc_skip{skip}", net, dev, lambda: [net(x)])
+        for name, shape in (("alex", (2, 3, 67, 93)), ("vgg", (2, 3, 64, 96))):
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore", UserWarning)      # no weight files: seeded untrained tensors below
+                net = LPIPS(name, gemm_path=gp)
+            net.load_state_dict(random_lpips_state_dict(name, seed=15), strict=True)
+            net = net.to(dev)
+            x0, x1 = rand(shape, 16).to(dev), rand(shape, 17).to(dev)
+            for normalize in (False, True):
+                a, b = (x0, x1) if normalize else (2 * x0 - 1, 2 * x1 - 1)    # [0, 1] with normalize, else [-1, 1]
+                case(out, f"gp{gp}/lpips_{name}_normalize{int(normalize)}", net, dev, lambda: lpips_fwd(net, a, b, normalize))
     print(json.dumps(out, indent=1))
 
 

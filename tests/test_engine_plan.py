@@ -1,6 +1,7 @@
 """CPU: the engine's plan - status, workspace bytes (with and without the semantic loss), decode workspace bytes and the
-FLOP count of one forward - for a grid of configurations.  femasr_net_create and these queries never touch a device, so
-the table pins the host-side graph (arena allocation order, launch list, taps that change the plan) without a GPU."""
+FLOP count of one forward - for a grid of configurations, and the status, workspace bytes and FLOP count of the
+discriminator and LPIPS handles.  The create calls and these queries never touch a device, so the tables pin the
+host-side graphs (arena allocation order, launch list, taps that change the plan) without a GPU."""
 import ctypes
 
 import pytest
@@ -270,6 +271,95 @@ def test_engine_plan(built_lib, name, gemm_path):
             assert g[5] is None
         else:
             assert g[5] == pytest.approx(fl, rel=1e-12, abs=0), shape
+
+
+HEAD_SHAPES = {
+    "disc": ((1, 64, 64), (2, 96, 160), (4, 256, 256), (1, 36, 40)),
+    "alex": ((1, 31, 31), (2, 67, 93), (8, 256, 256), (1, 30, 64)),
+    "vgg": ((1, 32, 48), (2, 64, 96), (8, 256, 256), (1, 24, 64)),
+}
+# name -> (shape table, skip_connection for the discriminator / net for LPIPS)
+HEADS = {"disc_skip": ("disc", 1), "disc_noskip": ("disc", 0), "lpips_alex": ("alex", 0), "lpips_vgg": ("vgg", 1)}
+
+
+def head_plan(L, name, gemm_path):
+    """The discriminator's or LPIPS' plan: {"BxHxW": [status, workspace bytes, flops]} (None where not defined)."""
+    kind, arg = HEADS[name]
+    h = ctypes.c_void_p()
+    if kind == "disc":
+        assert L.femasr_disc_create(ctypes.byref(lib.DiscConfig(3, 64, arg, gemm_path)), ctypes.byref(h)) == 0
+        ws, flops = L.femasr_disc_workspace_bytes, L.femasr_disc_flops
+    else:
+        assert L.femasr_lpips_create(ctypes.byref(lib.LpipsConfig(arg, gemm_path)), ctypes.byref(h)) == 0
+        ws, flops = L.femasr_lpips_workspace_bytes, L.femasr_lpips_flops
+    try:
+        out = {}
+        for (B, H, W) in HEAD_SHAPES[kind]:
+            n = ctypes.c_size_t()
+            s = ws(h, B, H, W, ctypes.byref(n))
+            out[f"{B}x{H}x{W}"] = [s, n.value if s == 0 else None, flops(h, B, H, W) if s == 0 else None]
+        return out
+    finally:
+        L.femasr_net_destroy(h)
+
+
+HEAD_EXPECTED = {
+    "disc_skip/gp0": {
+        "1x64x64": [0, 4194560, 3240099840.0],
+        "2x96x160": [0, 31457536, 24300748800.0],
+        "4x256x256": [0, 268435712, 207366389760.0],
+        "1x36x40": [-1, N, N],
+    },
+    "disc_skip/gp1": {
+        "1x64x64": [0, 4194560, 3240099840.0],
+        "2x96x160": [0, 31457536, 24300748800.0],
+        "4x256x256": [0, 268435712, 207366389760.0],
+        "1x36x40": [-1, N, N],
+    },
+    "disc_noskip/gp0": {
+        "1x64x64": [0, 4194560, 3240099840.0],
+        "2x96x160": [0, 31457536, 24300748800.0],
+        "4x256x256": [0, 268435712, 207366389760.0],
+        "1x36x40": [-1, N, N],
+    },
+    "disc_noskip/gp1": {
+        "1x64x64": [0, 4194560, 3240099840.0],
+        "2x96x160": [0, 31457536, 24300748800.0],
+        "4x256x256": [0, 268435712, 207366389760.0],
+        "1x36x40": [-1, N, N],
+    },
+    "lpips_alex/gp0": {
+        "1x31x31": [0, 176128, 24165120.0],
+        "2x67x93": [0, 2523648, 442712064.0],
+        "8x256x256": [0, 113799680, 27792070656.0],
+        "1x30x64": [-1, N, N],
+    },
+    "lpips_alex/gp1": {
+        "1x31x31": [0, 176128, 24165120.0],
+        "2x67x93": [0, 2523648, 442712064.0],
+        "8x256x256": [0, 113799680, 27792070656.0],
+        "1x30x64": [-1, N, N],
+    },
+    "lpips_vgg/gp0": {
+        "1x32x48": [0, 1573376, 1879179264.0],
+        "2x64x96": [0, 12583424, 15033434112.0],
+        "8x256x256": [0, 536871424, 641426522112.0],
+        "1x24x64": [-1, N, N],
+    },
+    "lpips_vgg/gp1": {
+        "1x32x48": [0, 1573376, 1879179264.0],
+        "2x64x96": [0, 12583424, 15033434112.0],
+        "8x256x256": [0, 536871424, 641426522112.0],
+        "1x24x64": [-1, N, N],
+    },
+}
+
+
+@pytest.mark.parametrize("gemm_path", [0, 1])
+@pytest.mark.parametrize("name", sorted(HEADS))
+def test_head_plan(built_lib, name, gemm_path):
+    got = head_plan(lib.load(), name, gemm_path)
+    assert got == HEAD_EXPECTED[f"{name}/gp{gemm_path}"]
 
 
 def test_in_conv_tap_changes_the_tensor_core_plan(built_lib):
