@@ -1129,6 +1129,8 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
   FEMASR_CHECK_ARG(a->ksize != 4 || stride == 2, "tc_igemm: ksize 4 needs stride 2");
   FEMASR_CHECK_ARG(a->ksize != 4 || (H >= 2 && W >= 2), "tc_igemm: a 4x4 stride-2 conv needs H, W >= 2");
   FEMASR_CHECK_ARG(a->ksize != 5 || (stride == 1 && !a->upsample), "tc_igemm: ksize 5 (pad 2) needs stride 1, no upsample");
+  // the 5x5 instantiations (EXT = 2) carry no LeakyReLU epilogue: refused rather than returned without the activation
+  FEMASR_CHECK_ARG(a->ksize != 5 || a->act != FEMASR_ACT_LRELU, "tc_igemm: no LeakyReLU epilogue for ksize 5");
   if (a->ksize == 1) { W = B * H * W; H = 1; B = 1; }     // pointwise: one long row of tokens
   const int Hin = H, Win = W;                             // activation-plane dims
   if (stride == 2) { H = (H + 2 - a->ksize) / 2 + 1; W = (W + 2 - a->ksize) / 2 + 1; }   // tiles run over the output grid

@@ -212,7 +212,7 @@ typedef struct {
   float* y;                /* fp32 NHWC [B,H,W,Cout] */
   int B, H, W, Cin, Cout;
   int ksize;               /* 1, 3 (pad 1), 4 (pad 1, stride 2 only) or 5 (pad 2, stride 1 only) */
-  int act;                 /* FEMASR_ACT_* */
+  int act;                 /* FEMASR_ACT_*; FEMASR_ACT_LRELU with ksize 5 or f8 is refused (FEMASR_ERR_ARG) */
   void* out_hi;            /* optional: write the result as split fp16 NHWC planes (the next GEMM's operand) */
   void* out_lo;            /*           instead of fp32 y (y may then be NULL) */
   int stride;              /* 0|1: stride 1.  2: 3x3 stride-2 conv (pad 1); H,W are the INPUT dims, y is

@@ -31,7 +31,7 @@ def pack_weight(w_oihw):
 
 
 def igemm(x, w_packed, bias, B, Hin, Win, Cin, Cout, ksize=3, stride=1, upsample=0, prologue=0, pro_a=None,
-          pro_b=None, gamma=None, beta=None, act=0, res1=None, res2=None, fn="femasr_igemm_simt"):
+          pro_b=None, gamma=None, beta=None, act=0, res1=None, res2=None, fn="femasr_igemm_simt", y=None):
     lib = L.load()
     He, We = (2 * Hin, 2 * Win) if upsample else (Hin, Win)
     if ksize == 1:
@@ -40,7 +40,8 @@ def igemm(x, w_packed, bias, B, Hin, Win, Cin, Cout, ksize=3, stride=1, upsample
         Ho, Wo = He, We
     else:
         Ho, Wo = (He - 1) // 2 + 1, (We - 1) // 2 + 1
-    y = torch.empty(B, Ho, Wo, Cout, device=x.device)
+    if y is None:
+        y = torch.empty(B, Ho, Wo, Cout, device=x.device)
     a = L.IgemmArgs(p(x), p(w_packed), p(bias), p(res1), p(res2), p(y), p(pro_a), p(pro_b), p(gamma), p(beta),
                     B, Hin, Win, Cin, Cout, ksize, stride, upsample, prologue, act)
     L.check(getattr(lib, fn)(C.byref(a), S()))
@@ -120,13 +121,16 @@ def tc_pack_up2(w_oihw):
 
 
 def tc_igemm(hi, lo, blob, bias, Cout, ksize=3, act=0, res1=None, res2=None, y=None, upsample=0, split_out=False,
-             gn_partial=None, stride=1, kb_begin=0, kb_count=0, slice_kb=0, pair=-1, strip=-1, f8=0):
+             gn_partial=None, stride=1, kb_begin=0, kb_count=0, slice_kb=0, pair=-1, strip=-1, f8=0, out_planes=None):
+    """out_planes: the caller's (hi, lo) output planes (implies split_out); y: the caller's fp32 output."""
     lib = L.load()
     B, H, W, Cin = hi.shape
     u = 2 if upsample else 1
-    Ho, Wo = ((H - 1) // 2 + 1, (W - 1) // 2 + 1) if stride == 2 else (H * u, W * u)
+    Ho, Wo = ((H + 2 - ksize) // 2 + 1, (W + 2 - ksize) // 2 + 1) if stride == 2 else (H * u, W * u)
     oh = ol = None
-    if split_out:
+    if out_planes is not None:
+        (oh, ol), split_out = out_planes, True
+    elif split_out:
         oh = torch.empty(B, Ho, Wo, Cout, dtype=torch.float16, device=hi.device)
         ol = torch.empty_like(oh)
     elif y is None:
