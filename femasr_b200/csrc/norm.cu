@@ -6,7 +6,14 @@ namespace femasr {
 constexpr int GN_GROUPS = 32;
 constexpr int GN_CHUNK = 512;   // pixels per partial block
 
-// partial[b][chunk][g][2] = (sum, sumsq) over `GN_CHUNK` pixels x (C/32) channels, fp32 per thread then
+// The sums are taken about a shift K per (image, group), the group's first channel at the image's first pixel: the fp32
+// sum of squares of x itself would round away var / mean^2 of its own precision, so a2 / n - mean^2 loses (mean / std)^2
+// ulps; about K it loses ((mean - K) / std)^2 instead, and K is a sample of the group.
+__device__ __forceinline__ const float* gn_shift_ptr(const float* x, int b, int HW, int C, int g) {
+  return x + (long)b * HW * C + g * (C / GN_GROUPS);
+}
+
+// partial[b][chunk][g][2] = (sum, sumsq) of x - K over `GN_CHUNK` pixels x (C/32) channels, fp32 per thread then
 // combined in double in a fixed order.
 __global__ void __launch_bounds__(256) gn_partial_kernel(const float* __restrict__ x, double* __restrict__ partial,
                                                          int HW, int C, int nchunks) {
@@ -17,13 +24,18 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const float* __restrict
   const int q = threadIdx.x % quads, lane = threadIdx.x / quads;
   const int p0 = chunk * GN_CHUNK;
   const int p1 = min(p0 + GN_CHUNK, HW);
+  // the quad's channels 4q..4q+3 lie in one group for cpg 4 and 8, in two (4q, 4q+2) for cpg 2
+  const int cpg = C / GN_GROUPS;
+  const float ka = __ldg(gn_shift_ptr(x, b, HW, C, 4 * q / cpg));
+  const float kb = cpg == 2 ? __ldg(gn_shift_ptr(x, b, HW, C, 4 * q / 2 + 1)) : ka;
   float s[4] = {0.f, 0.f, 0.f, 0.f}, ss[4] = {0.f, 0.f, 0.f, 0.f};
   const float* base = x + ((long)b * HW) * C + q * 4;
   for (int p = p0 + lane; p < p1; p += lanes) {
     const float4 v = __ldg(reinterpret_cast<const float4*>(base + (long)p * C));
-    s[0] += v.x; s[1] += v.y; s[2] += v.z; s[3] += v.w;
-    ss[0] = fmaf(v.x, v.x, ss[0]); ss[1] = fmaf(v.y, v.y, ss[1]);
-    ss[2] = fmaf(v.z, v.z, ss[2]); ss[3] = fmaf(v.w, v.w, ss[3]);
+    const float d0 = v.x - ka, d1 = v.y - ka, d2 = v.z - kb, d3 = v.w - kb;
+    s[0] += d0; s[1] += d1; s[2] += d2; s[3] += d3;
+    ss[0] = fmaf(d0, d0, ss[0]); ss[1] = fmaf(d1, d1, ss[1]);
+    ss[2] = fmaf(d2, d2, ss[2]); ss[3] = fmaf(d3, d3, ss[3]);
   }
 #pragma unroll
   for (int i = 0; i < 4; ++i) { red[threadIdx.x][i] = s[i]; red[threadIdx.x][4 + i] = ss[i]; }
@@ -45,9 +57,10 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const float* __restrict
 }
 
 // one warp per (b, group): reduce partials, then write the folded scale/shift for its channels.
-__global__ void gn_finalize_kernel(const double* __restrict__ partial, const float* __restrict__ gamma,
-                                   const float* __restrict__ beta, float* __restrict__ scale,
-                                   float* __restrict__ shift, int HW, int C, int nchunks, float eps) {
+__global__ void gn_finalize_kernel(const float* __restrict__ x, const double* __restrict__ partial,
+                                   const float* __restrict__ gamma, const float* __restrict__ beta,
+                                   float* __restrict__ scale, float* __restrict__ shift, int HW, int C, int nchunks,
+                                   float eps) {
   const int b = blockIdx.x, g = threadIdx.x >> 5, lane = threadIdx.x & 31;
   double a = 0.0, a2 = 0.0;
   for (int ch = lane; ch < nchunks; ch += 32) {
@@ -57,8 +70,9 @@ __global__ void gn_finalize_kernel(const double* __restrict__ partial, const flo
   a = warp_sum_d(a); a2 = warp_sum_d(a2);
   const int cpg = C / GN_GROUPS;
   const double n = (double)HW * cpg;
-  const double mean = a / n;
-  double var = a2 / n - mean * mean;
+  const double dm = a / n;                                    // mean of x - K
+  const double mean = (double)__ldg(gn_shift_ptr(x, b, HW, C, g)) + dm;
+  double var = a2 / n - dm * dm;
   if (var < 0.0) var = 0.0;
   const float rstd = (float)(1.0 / sqrt(var + (double)eps));
   const float meanf = (float)mean;
@@ -158,7 +172,7 @@ extern "C" int femasr_gn_stats(const float* x, const float* gamma, const float* 
   gn_partial_kernel<<<dim3(nchunks, B), 256, 0, as_stream(stream)>>>(x, partial, HW, C, nchunks);
   int st = launch_status("gn_partial_kernel");
   if (st) return st;
-  gn_finalize_kernel<<<B, GN_GROUPS * 32, 0, as_stream(stream)>>>(partial, gamma, beta, scale, shift, HW, C, nchunks, eps);
+  gn_finalize_kernel<<<B, GN_GROUPS * 32, 0, as_stream(stream)>>>(x, partial, gamma, beta, scale, shift, HW, C, nchunks, eps);
   return launch_status("gn_finalize_kernel");
 }
 
