@@ -26,6 +26,8 @@ from torch import nn
 
 from basicsr.utils.registry import ARCH_REGISTRY
 from femasr_b200.lib import FemasrError
+from femasr_b200.module import EngineModule, attach
+from femasr_b200.module import Node as _Node  # noqa: F401  (whole-module pickles name the containers by this path)
 from femasr_b200.net import NativeNet
 from femasr_b200.spec import (VGG_CONVS, VGG_TORCHVISION_INDEX, normalize_codebooks, param_spec, relative_position_index,
                               shift_attn_mask, vgg_init)
@@ -44,25 +46,6 @@ def _vgg_pretrained():
         for t in ("weight", "bias"):
             out[f"vgg_feat_extractor.vgg_net.{name}.{t}"] = sd[f"features.{i}.{t}"].detach().float().clone()
     return out
-
-
-class _Node(nn.Module):
-    """A bare container; the tree of these reproduces the reference's dotted parameter names."""
-
-
-def _attach(root: nn.Module, dotted: str, tensor: torch.Tensor, buffer: bool):
-    *path, leaf = dotted.split(".")
-    node = root
-    for part in path:
-        nxt = node._modules.get(part)
-        if nxt is None:
-            nxt = _Node()
-            node.add_module(part, nxt)
-        node = nxt
-    if buffer:
-        node.register_buffer(leaf, tensor)
-    else:
-        node.register_parameter(leaf, nn.Parameter(tensor, requires_grad=False))
 
 
 def _init_tensor(shape, kind: str, fan_in: int, n_e: int) -> torch.Tensor:
@@ -84,11 +67,11 @@ def _init_tensor(shape, kind: str, fan_in: int, n_e: int) -> torch.Tensor:
 
 
 @ARCH_REGISTRY.register()
-class FeMaSRNet(nn.Module):
+class FeMaSRNet(EngineModule):
     def __init__(self, *, in_channel=3, codebook_params=None, gt_resolution=256, LQ_stage=False,
                  norm_type='gn', act_type='silu', use_quantize=True, scale_factor=4,
                  use_semantic_loss=False, use_residual=True, **ignore_kwargs):
-        super().__init__()
+        super().__init__(ignore_kwargs.get("gemm_path", -1))
         cb = np.array(codebook_params)
         if cb.ndim != 2 or cb.shape[1] != 3:
             raise ValueError("codebook_params must be [[scale, n_e, e_dim], ...]")
@@ -117,7 +100,6 @@ class FeMaSRNet(nn.Module):
         self.use_semantic_loss = bool(use_semantic_loss)     # may be toggled like the reference's test() does (:451-452)
         self._semantic_params = bool(use_semantic_loss)      # whether conv_semantic / vgg_feat_extractor exist
         self.max_depth = int(np.log2(gt_resolution // self.codebook_scale[0]))
-        self.gemm_path = int(ignore_kwargs.get("gemm_path", -1))    # -1: engine default
 
         vgg = None
         if self._semantic_params:
@@ -129,75 +111,22 @@ class FeMaSRNet(nn.Module):
         for name, shape, kind, fan_in in param_spec(self.scale_factor, self.e_dim, self.n_e, in_channel,
                                                     codebooks=self.codebooks, semantic=self._semantic_params):
             if kind == "rpi":
-                _attach(self, name, relative_position_index(), buffer=True)
+                attach(self, name, relative_position_index(), buffer=True)
             elif kind == "mask":
-                _attach(self, name, shift_attn_mask(32, 32), buffer=True)
+                attach(self, name, shift_attn_mask(32, 32), buffer=True)
             elif kind in ("vgg_mean", "vgg_std"):
-                _attach(self, name, vgg_init(shape, kind, fan_in), buffer=True)
+                attach(self, name, vgg_init(shape, kind, fan_in), buffer=True)
             elif kind in ("vgg_w", "vgg_b"):
                 t = vgg[name] if vgg is not None else vgg_init(shape, kind, fan_in)
                 if tuple(t.shape) != tuple(shape):
                     raise ValueError(f"{VGG_PRETRAIN_PATH}: {name} has shape {tuple(t.shape)}, expected {tuple(shape)}")
-                _attach(self, name, t, buffer=False)
+                attach(self, name, t, buffer=False)
             else:
-                _attach(self, name, _init_tensor(shape, kind, fan_in, fan_in), buffer=False)   # codebook: fan_in = its n_e
-        self._engine = None
-        self._engine_sig = None
-        self._plist = None
+                attach(self, name, _init_tensor(shape, kind, fan_in, fan_in), buffer=False)   # codebook: fan_in = its n_e
 
-    # ------------------------------------------------------------------ engine plumbing
-    def _float_params(self):
-        return {k: v for k, v in self.state_dict(keep_vars=True).items() if v.dtype == torch.float32
-                and not k.endswith("attn_mask")}
-
-    def _param_list(self):
-        """(name, tensor) pairs of the engine's parameters, cached: walking state_dict() costs ~1 ms per call (437
-        tensors), which the reference's batch-1 loop would pay per image.  Invalidated whenever the tensor OBJECTS may
-        have been replaced: `_apply` (.to/.cuda/.float/...), `load_state_dict`."""
-        if self._plist is None:
-            self._plist = list(self._float_params().items())
-        return self._plist
-
-    def _apply(self, fn, *a, **kw):
-        out = super()._apply(fn, *a, **kw)
-        self._plist = None
-        return out
-
-    def load_state_dict(self, *a, **kw):
-        out = super().load_state_dict(*a, **kw)
-        self._plist = None
-        self._engine_sig = None
-        return out
-
-    def refresh_weights(self):
-        """Force a re-upload of the parameters on the next call.  Needed only after in-place surgery that bypasses
-        autograd's version counter (`p.data.copy_(...)`, e.g. BasicSR's model_ema): `(data_ptr, _version)` is how
-        changes are detected, and `.data` writes do not bump `_version`."""
-        self._plist = None
-        self._engine_sig = None
-
-    def _native(self, device: torch.device) -> NativeNet:
-        """The engine with the module's CURRENT parameter values (re-uploaded when they change)."""
-        from femasr_b200 import default_gemm_path
-        plist = self._param_list()
-        sig = tuple((v.data_ptr(), v._version) for _k, v in plist)      # ~0.07 ms (was ~1.1 ms through state_dict())
-        if self._engine is None:
-            gp = self.gemm_path if self.gemm_path >= 0 else default_gemm_path()
-            self._engine = NativeNet(self.scale_factor, self.n_e, self.e_dim, self.use_quantize,
-                                     self.use_residual, gemm_path=gp, codebooks=self.codebooks,
-                                     use_semantic_loss=self._semantic_params)
-        if sig != self._engine_sig:
-            self._engine.load_state_dict(dict(plist), device)
-            self._engine_sig = sig
-        return self._engine
-
-    def __getstate__(self):
-        # the engine is a process-local native handle: copies / pickles rebuild it lazily from the parameters
-        state = self.__dict__.copy()
-        state["_engine"] = None
-        state["_engine_sig"] = None
-        state["_plist"] = None
-        return state
+    def _make_engine(self, gemm_path: int) -> NativeNet:
+        return NativeNet(self.scale_factor, self.n_e, self.e_dim, self.use_quantize, self.use_residual,
+                         gemm_path=gemm_path, codebooks=self.codebooks, use_semantic_loss=self._semantic_params)
 
     # ------------------------------------------------------------------ reference surface
     def encode_and_decode(self, input, gt_indices=None, current_iter=None):

@@ -2,6 +2,7 @@
 
   femasr_b200.lib    ctypes binding of libfemasr_b200.so (C ABI in include/femasr_b200.h)
   femasr_b200.net    host engine wrapper (workspace, test()/test_tile() scheduling)
+  femasr_b200.module nn.Module base of the engine-backed networks (tensor tree, upload on change)
   femasr_b200.spec   parameter inventory + seeded random weights
   femasr_b200.build  nvcc build of the library (in-tree)
 The reference-facing operator surface lives in `basicsr.archs.femasr_arch.FeMaSRNet`.

@@ -20,26 +20,11 @@ import warnings
 from typing import Dict, Optional
 
 import torch
-from torch import nn
 
 from .lib import FemasrError
+from .module import EngineModule, attach
 from .net import NativeLPIPS
 from .spec import LPIPS_CONVS, lpips_spec, random_lpips_state_dict
-
-
-def _attach(root: nn.Module, dotted: str, tensor: torch.Tensor, buffer: bool):
-    *path, leaf = dotted.split(".")
-    node = root
-    for part in path:
-        child = node._modules.get(part)
-        if child is None:
-            child = nn.Module()
-            node.add_module(part, child)
-        node = child
-    if buffer:
-        node.register_buffer(leaf, tensor)
-    else:
-        node.register_parameter(leaf, nn.Parameter(tensor, requires_grad=False))
 
 
 def backbone_from_torchvision(net: str, sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
@@ -64,7 +49,7 @@ def lins_from_lpips(net: str, sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Te
     return {k: sd[k] for k in want}
 
 
-class LPIPS(nn.Module):
+class LPIPS(EngineModule):
     """The `lpips` package's LPIPS(net=net) (v0.1, lpips=True, spatial=False) in eval mode on the engine.
 
     backbone_path: a torchvision alexnet / vgg16 checkpoint (features.{i}.*); lin_path: an lpips lin-weights file
@@ -73,14 +58,13 @@ class LPIPS(nn.Module):
     def __init__(self, net: str = "alex", gemm_path: int = -1, version: str = "0.1", lpips: bool = True,
                  spatial: bool = False, backbone_path: Optional[str] = None, lin_path: Optional[str] = None,
                  **ignore_kwargs):
-        super().__init__()
+        super().__init__(gemm_path)
         if net not in ("alex", "vgg"):
             raise NotImplementedError(f"femasr_b200 computes LPIPS with net='alex' or 'vgg'; got net={net!r}")
         if version != "0.1" or not lpips or spatial:
             raise NotImplementedError("femasr_b200 computes LPIPS v0.1 with lpips=True and spatial=False only; got "
                                       f"version={version!r}, lpips={lpips}, spatial={spatial}")
         self.pnet_type = net
-        self.gemm_path = int(gemm_path)
         tensors = random_lpips_state_dict(net)
         if backbone_path is None or lin_path is None:
             warnings.warn(f"LPIPS({net!r}): no {'backbone' if backbone_path is None else 'lin'} weight file given; "
@@ -91,34 +75,11 @@ class LPIPS(nn.Module):
         if lin_path is not None:
             tensors.update(lins_from_lpips(net, torch.load(lin_path, map_location="cpu")))
         for name, _shape, kind, _f in lpips_spec(net):
-            _attach(self, name, tensors[name].float().contiguous(), buffer=kind in ("shift", "scale"))
-        self._engine = None
-        self._engine_sig = None
+            attach(self, name, tensors[name].float().contiguous(), buffer=kind in ("shift", "scale"))
         self.eval()
 
-    def load_state_dict(self, *a, **kw):
-        out = super().load_state_dict(*a, **kw)
-        self._engine_sig = None
-        return out
-
-    def __getstate__(self):
-        # the engine is a process-local native handle: copies / pickles rebuild it lazily from the tensors
-        state = self.__dict__.copy()
-        state["_engine"] = None
-        state["_engine_sig"] = None
-        return state
-
-    def _native(self, device: torch.device) -> NativeLPIPS:
-        """The engine with the module's CURRENT tensors (re-uploaded when a (data_ptr, _version) changes)."""
-        from femasr_b200 import default_gemm_path
-        tensors = self.state_dict(keep_vars=True)
-        sig = tuple((v.data_ptr(), v._version) for v in tensors.values())
-        if self._engine is None:
-            self._engine = NativeLPIPS(self.pnet_type, self.gemm_path if self.gemm_path >= 0 else default_gemm_path())
-        if sig != self._engine_sig:
-            self._engine.load_state_dict(tensors, device)
-            self._engine_sig = sig
-        return self._engine
+    def _make_engine(self, gemm_path: int) -> NativeLPIPS:
+        return NativeLPIPS(self.pnet_type, gemm_path)
 
     @torch.no_grad()
     def forward(self, in0, in1, retPerLayer=False, normalize=False):

@@ -51,8 +51,14 @@ def padded_size(n: int, scale: int) -> int:
 
 class _Engine:
     """What every engine handle shares: creation on first use on a CUDA device, the parameter upload by reference name,
-    the device workspace and the per-kernel profile.  Subclasses set ``lib``, ``_h``, ``_ws``, ``device``, ``names``
-    and implement ``_create``."""
+    the device workspace and the per-kernel profile.  Subclasses pass the names they upload and implement ``_create``."""
+
+    def __init__(self, names: List[str]):
+        self.lib = L.load()
+        self._h = C.c_void_p()
+        self._ws: Optional[torch.Tensor] = None
+        self.device: Optional[torch.device] = None
+        self.names = names
 
     def _create(self):
         raise NotImplementedError
@@ -128,7 +134,6 @@ class NativeNet(_Engine):
         variant (femasr_arch.py:231-235); default one codebook (32, n_e, e_dim).  ``use_semantic_loss``: the engine also
         holds the VGG19 / conv_semantic tensors (femasr_arch.py:301-309) and forward(want_sem=True) computes the HQ
         stage's semantic loss."""
-        self.lib = L.load()
         self.scale = int(scale_factor)
         self.codebooks = normalize_codebooks(codebooks, n_e, e_dim)
         self.n_e, self.e_dim = self.codebooks[0][1], self.codebooks[0][2]
@@ -137,14 +142,10 @@ class NativeNet(_Engine):
         self.cfg = L.NetConfig(self.scale, self.n_e, self.e_dim, 3, int(bool(use_quantize)),
                                int(bool(use_residual)), int(gemm_path), K, pad([c[0] for c in self.codebooks]),
                                pad([c[1] for c in self.codebooks]), pad([c[2] for c in self.codebooks]))
-        self._h = C.c_void_p()
-        self._ws: Optional[torch.Tensor] = None
-        self._taps: Dict[str, torch.Tensor] = {}
-        self.device: Optional[torch.device] = None
         self.use_semantic_loss = bool(use_semantic_loss)
-        self.names = [n for (n, _s, kind, _f) in param_spec(self.scale, self.e_dim, self.n_e, codebooks=self.codebooks,
-                                                             semantic=self.use_semantic_loss)
-                      if kind not in ("rpi", "mask")]
+        super().__init__([n for (n, _s, kind, _f) in param_spec(self.scale, self.e_dim, self.n_e, codebooks=self.codebooks,
+                                                                semantic=self.use_semantic_loss)
+                          if kind not in ("rpi", "mask")])
         # the forward is a fixed launch list per input shape: replay it as a CUDA graph (no per-launch host work)
         self.use_graph = os.environ.get("FEMASR_CUDA_GRAPH", "1") != "0"
         # Captured graphs pin their workspace and static buffers (13 GB at 32x128x128), so the cache is a small LRU and
@@ -398,12 +399,8 @@ class NativeDisc(_Engine):
     """UNetDiscriminatorSN (discriminator_arch.py) on the engine: forward(x [B,3,H,W]) -> [B,1,H,W], eval mode."""
 
     def __init__(self, skip_connection: bool = True, gemm_path: int = 0, num_in_ch: int = 3, num_feat: int = 64):
-        self.lib = L.load()
+        super().__init__([n for (n, _s, _k, _f) in disc_spec(num_in_ch, num_feat)])
         self.dcfg = L.DiscConfig(int(num_in_ch), int(num_feat), int(bool(skip_connection)), int(gemm_path))
-        self._h = C.c_void_p()
-        self._ws: Optional[torch.Tensor] = None
-        self.device: Optional[torch.device] = None
-        self.names = [n for (n, _s, _k, _f) in disc_spec(num_in_ch, num_feat)]
 
     def _create(self):
         L.check(self.lib.femasr_disc_create(C.byref(self.dcfg), C.byref(self._h)))
@@ -431,13 +428,9 @@ class NativeLPIPS(_Engine):
     """LPIPS v0.1 (the lpips package, net 'alex' | 'vgg') on the engine: forward(x0, x1) -> (d [B], r [5, B])."""
 
     def __init__(self, net: str = "alex", gemm_path: int = 0):
-        self.lib = L.load()
+        super().__init__([n for (n, _s, _k, _f) in lpips_spec(net)])
         self.net = net
         self.lcfg = L.LpipsConfig({"alex": 0, "vgg": 1}[net], int(gemm_path))
-        self._h = C.c_void_p()
-        self._ws: Optional[torch.Tensor] = None
-        self.device: Optional[torch.device] = None
-        self.names = [n for (n, _s, _k, _f) in lpips_spec(net)]
 
     def _create(self):
         L.check(self.lib.femasr_lpips_create(C.byref(self.lcfg), C.byref(self._h)))
