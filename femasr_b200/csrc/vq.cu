@@ -64,13 +64,20 @@ __global__ void __launch_bounds__(256) vq_select_kernel(const float* __restrict_
 // candidate inside the margin gets its distance recomputed with an exact dot product (fp64 accumulate, rounded once:
 // what "any fp32-accurate z.e" of SURVEY 7.3-2 asks for) through the reference's rounding sequence
 // fl(fl(A + B_j) - 2 C_j) and the lowest-index tie rule; if even the fourth candidate is inside the margin the whole
-// codebook is rescanned exactly.  The tensor-core distance differs from the exact one by at most one grid step
-// (|dC| ~ 1e-8 against ulp(A) ~ 3e-5), so the true argmin is always within 2 steps of the tensor-core best.
+// codebook is rescanned exactly.
 // Then: gather, straight-through residual z + (e - z), per-row loss (femasr_arch.py:67-100).
-// Margin.  With u = the grid step of the fp32 distance formula (ulp of max(A + B, d): the subtraction may cancel) and a
-// tensor-core error of 2C far below u, tensor-core and exact distance of one code differ by at most u, so the true
-// argmin (and every exact tie with a lower index) lies within 2u of the tensor-core best: 2.5 u is used, plus four times a
-// bound of the tensor-core error of 2C itself (3 * e_dim / 16 truncating accumulations of <= 1 ulp each).
+// Margin.  With u = the grid step of the fp32 distance formula (ulp of max(A + B, d): the subtraction may cancel),
+// tensor-core and exact distance of code j differ by at most u + |2 dC_j|, so the true argmin (and every exact tie with
+// a lower index) lies within 2u + |2 dC_best| + |2 dC_argmin| of the tensor-core best.  The margin is 2.5 u plus two
+// bounds of the tensor-core error of 2C:
+//   * relative: four times 3 * e_dim / 16 truncating accumulations of <= 1 ulp each of 2C;
+//   * absolute: z is split into fp16 hi / lo planes without a scale, so below |z| ~ 2^-3 the lo plane is subnormal and
+//     each z_k carries up to 2^-25 of absolute error whatever its size.  By Cauchy-Schwarz that moves 2 C_j by at most
+//     2^-24 * sqrt(e_dim * B_j); twice that (the best code and the true argmin), taken at the largest B_j of the four
+//     candidates.  A code outside the list escapes this only if its norm exceeds all four candidates' and its exact
+//     distance beats them all.
+// The grid step u shrinks as |z|^2 while the absolute term does not: for z of std 2^-12 the absolute term is ~2000 u,
+// for z of std ~1 it is ~1e-3 u.
 constexpr float VQ_MARGIN_ULPS = 2.5f;
 __device__ __forceinline__ float ulp_of(float x) {      // spacing of fp32 numbers at |x| (normal range)
   return __uint_as_float(__float_as_uint(x) & 0x7f800000u) * 1.1920929e-7f;
@@ -107,8 +114,12 @@ __global__ void __launch_bounds__(256) vq_finish_kernel(const float* __restrict_
   } else {
     const float ar0 = a[r];
     const float ab0 = ar0 + __ldg(esq + bj);
+    float bmax = __ldg(esq + bj);
+#pragma unroll
+    for (int k = 1; k < 4; ++k) if (j[k] != 0x7fffffff) bmax = fmaxf(bmax, __ldg(esq + j[k]));
     const float margin = VQ_MARGIN_ULPS * ulp_of(fmaxf(fabsf(ab0), fabsf(d[0]))) +
-                         4.0f * 1.1920929e-7f * (float)(3 * e_dim / 16) * fabsf(ab0 - d[0]) + 1e-30f;
+                         4.0f * 1.1920929e-7f * (float)(3 * e_dim / 16) * fabsf(ab0 - d[0]) +
+                         0x1p-23f * sqrtf((float)e_dim * bmax) + 1e-30f;
     int nc = 1;
 #pragma unroll
     for (int k = 1; k < 4; ++k) nc += (j[k] != 0x7fffffff && d[k] - d[0] <= margin) ? 1 : 0;   // ascending: a prefix
