@@ -31,9 +31,20 @@ struct Arena {
   size_t top = 0, peak = 0, cap = 0;
   bool dry = true;
   bool overflow = false;      // real run only: an allocation ran past the caller's workspace (sizing bug) - never launch on it
+  int poison = -1;            // real run only: femasr_net_set_poison's byte, memset over every block as it is handed out
+  cudaStream_t st = nullptr;  // the run's stream (the poison memsets)
+  cudaError_t poison_err = cudaSuccess;
   static size_t align(size_t n) { return (n + 255) & ~size_t(255); }
   size_t alloc_off(size_t bytes) {
     bytes = align(std::max<size_t>(bytes, 256));
+    const size_t off = place(bytes);
+    if (poison >= 0 && !dry && off + bytes <= cap) {
+      const cudaError_t e = cudaMemsetAsync(base + off, poison, bytes, st);
+      if (poison_err == cudaSuccess) poison_err = e;
+    }
+    return off;
+  }
+  size_t place(size_t bytes) {
     for (size_t i = 0; i < blks.size(); ++i) {
       if (blks[i].free && blks[i].size >= bytes) {
         if (blks[i].size > bytes) {
@@ -124,6 +135,7 @@ struct femasr_net {
   std::map<std::string, Tap> taps;
   int last_launches = 0;
   bool profile = false;
+  int poison = -1;                        // femasr_net_set_poison: byte every workspace block is filled with, -1 = off
   bool tc_precise = true;                 // K-sliced fp32 accumulation for the layers in front of the VQ
   bool f8_cross = true;                   // layers behind the VQ: the two cross products of the split as one fp8 product (FEMASR_F8_CROSS=0: three fp16 products)
   int tc_slice_kb = 4;                    // K-slice length in 64-wide k-blocks (FEMASR_TC_SLICE_KB; study knob)
@@ -374,6 +386,8 @@ struct Ctx {
     ar.dry = !workspace;
     ar.base = ar.dry ? reinterpret_cast<char*>(uintptr_t(1) << 40) : reinterpret_cast<char*>(workspace) + mis;
     ar.cap = ar.dry ? 0 : bytes - mis;
+    ar.poison = ar.dry ? -1 : n->poison;
+    ar.st = st;
   }
   bool dry() const { return ar.dry; }
   bool ok() const { return status == FEMASR_OK; }
@@ -381,6 +395,7 @@ struct Ctx {
   size_t bytes_needed() const { return ar.peak + 256; }
   int finish() {
     if (!dry()) net->last_launches = (int)(g_launches - l0);
+    if (ar.poison_err != cudaSuccess) check(fail(FEMASR_ERR_CUDA, std::string("poison memset: ") + cudaGetErrorString(ar.poison_err)));
     return status;
   }
 
@@ -1374,6 +1389,13 @@ extern "C" int femasr_net_set_profile(femasr_net* net, int enable) {
   for (auto& r : net->prof) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
   net->prof.clear();
   net->profile = enable != 0;
+  return FEMASR_OK;
+}
+
+extern "C" int femasr_net_set_poison(femasr_net* net, int byte) {
+  FEMASR_CHECK_ARG(net, "set_poison: null");
+  FEMASR_CHECK_ARG(byte >= -1 && byte <= 255, "set_poison: byte must be -1 (off) or 0 ... 255");
+  net->poison = byte;
   return FEMASR_OK;
 }
 

@@ -85,6 +85,7 @@ SIGNATURES = {
     "femasr_net_last_launch_count": (_I, [_V]),
     "femasr_net_set_profile": (_I, [_V, _I]),
     "femasr_net_profile_json": (C.c_char_p, [_V]),
+    "femasr_net_set_poison": (_I, [_V, _I]),
     "femasr_net_flops": (_D, [_V, _I, _I, _I]),
     "femasr_flip_pad": (_I, [_V, _V, _I, _I, _I, _I, _I, _I, _V]),
     "femasr_u8_to_input": (_I, [_V, _V, _I, _I, _I, _I, _I, _V]),

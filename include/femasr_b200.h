@@ -126,6 +126,12 @@ int femasr_net_last_launch_count(femasr_net* net);
  * {"kernel": {"launches": n, "ms": total, "flops": algorithmic total}, ...} (valid until the next call). */
 int femasr_net_set_profile(femasr_net* net, int enable);
 const char* femasr_net_profile_json(femasr_net* net);
+/* Testing aid for every handle kind (generator, discriminator, LPIPS): with byte in [0, 255], every workspace block a
+ * forward / decode hands out is memset to `byte` on the run's stream before its first use, so a kernel that reads an
+ * element it did not write in this call sees that byte instead of what an earlier layer or call left there.  -1 (the
+ * default) turns it off.  Sizing queries, launch counts and the profile are unaffected; under CUDA graph capture the
+ * memsets become memset nodes.  Other values: FEMASR_ERR_ARG. */
+int femasr_net_set_poison(femasr_net* net, int byte);
 /* Algorithmic FLOPs (2*MAC, conv+linear+QK/PV+VQ distance) of one forward on [B,3,H,W]. */
 double femasr_net_flops(femasr_net* net, int B, int H, int W);
 

@@ -64,6 +64,25 @@ def test_argument_validation_without_gpu(built_lib):
     assert L.femasr_net_create(ctypes.byref(cfg), ctypes.byref(h)) == -1            # scales must increase
 
 
+def test_set_poison_range_without_gpu(built_lib):
+    """femasr_net_set_poison takes -1 (off) or one byte value, on every handle kind, and needs no device."""
+    from femasr_b200 import lib
+    L = lib.load()
+    assert L.femasr_net_set_poison(None, 0) == -1
+    for create, cfg in ((L.femasr_net_create, lib.NetConfig(4, 1024, 256, 3, 1, 1, 1)),
+                        (L.femasr_disc_create, lib.DiscConfig(3, 64, 1, 0)), (L.femasr_lpips_create, lib.LpipsConfig(1, 1))):
+        h = ctypes.c_void_p()
+        assert create(ctypes.byref(cfg), ctypes.byref(h)) == 0
+        try:
+            for bad in (256, -2, 1 << 30, -(1 << 30)):
+                assert L.femasr_net_set_poison(h, bad) == -1
+                assert b"set_poison" in L.femasr_last_error()
+            for good in (0, 0x41, 255, -1):
+                assert L.femasr_net_set_poison(h, good) == 0
+        finally:
+            L.femasr_net_destroy(h)
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
 def test_no_cpu_fallback(built_lib):
     from basicsr.archs.femasr_arch import FeMaSRNet
