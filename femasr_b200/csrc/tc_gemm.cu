@@ -183,17 +183,31 @@ constexpr int A_PLANE_BYTES = TC_BM * TC_BK * 2;   // 16 KB
 constexpr int TC_CONSUMER_WARPS = 8, TC_THREADS = 32 * TC_CONSUMER_WARPS + 32;
 constexpr int TC_SMEM_LIMIT = 232448;              // 227 KB of opt-in shared memory per block on H100
 
-template <int BN>
+// Column schedule (COLS): 8 x 16 output tiles; one activation box of 64 ch x 8 cols x 18 rows per (channel chunk, dx)
+// serves the three taps dy = -1, 0, +1 of that column, tap dy reading it from row 8 (dy + 1), i.e. 1024 (dy + 1) bytes
+// in: every wgmma start address stays on a 1024-byte swizzle atom.
+constexpr int COL_WT = 8, COL_HT = 16;
+constexpr int COL_PLANE_BYTES = (COL_HT + 2) * COL_WT * TC_BK * 2;   // 18 KB
+constexpr int COL_STAGE_BYTES = 2 * COL_PLANE_BYTES;                 // a_hi, a_lo8
+
+// Shared memory: [COLS: activation column ring][stage ring][barriers][GroupNorm partials].  Without COLS a stage holds
+// all four operand boxes of a k-block; with COLS it holds the two weight boxes and the activation columns have a ring of
+// their own.
+template <int BN, bool COLS = false>
 struct TcCfg {
   static_assert(BN == 64 || BN == 128, "tile width");
   static constexpr int B_PLANE_BYTES = BN * TC_BK * 2;
-  static constexpr int STAGE_BYTES = 2 * A_PLANE_BYTES + 2 * B_PLANE_BYTES;        // a_hi, a_lo, w_hi, w_lo
+  static constexpr int STAGE_BYTES = (COLS ? 0 : 2 * A_PLANE_BYTES) + 2 * B_PLANE_BYTES;   // (a_hi, a_lo,) w_hi, w_lo
+  static constexpr int COL_STAGES = COLS ? 2 : 0;
+  static constexpr int COL_RING_BYTES = COL_STAGES * COL_STAGE_BYTES;
   static constexpr int RED_BYTES = TC_CONSUMER_WARPS * 64 * 2 * 4;                  // per-warp GroupNorm partials
-  static constexpr int STAGES = (TC_SMEM_LIMIT - 1024 - 256 - RED_BYTES) / STAGE_BYTES;   // 3 (BN 128) / 4 (BN 64)
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + RED_BYTES;
+  // 3 (BN 128) / 4 (BN 64); COLS: 4 (BN 128) / 9 (BN 64)
+  static constexpr int STAGES = (TC_SMEM_LIMIT - 1024 - 256 - RED_BYTES - COL_RING_BYTES) / STAGE_BYTES;
+  static constexpr int RING_BYTES = COL_RING_BYTES + STAGES * STAGE_BYTES;
+  static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + RED_BYTES;
   static constexpr int NF = BN / 2;                                                  // accumulator floats per thread
   static_assert(SMEM_BYTES <= TC_SMEM_LIMIT, "shared memory budget");
-  static_assert(16 * STAGES <= 256, "barrier area");
+  static_assert(16 * (STAGES + COL_STAGES) <= 256, "barrier area");
 };
 
 // running top-4 of (d, j), ascending lexicographically; precondition: (d, j) sorts before (td[3], tj[3])
@@ -215,19 +229,25 @@ __device__ __forceinline__ void top4_insert(float (&td)[4], int (&tj)[4], float 
 // EXT: taps and epilogues beyond the generator's.  1: the discriminator's 4x4 taps and LeakyReLU epilogue; 2: LPIPS'
 // 5x5 pad-2 taps (AlexNet conv2).  A template parameter so that the other instantiations keep exactly the instruction
 // stream they had without them (measured: 1.3% slower GEMMs otherwise).
-template <int BN, bool RES, bool F8, bool VQ = false, int EXT = 0>
+// COLS: the column schedule (TcCfg) of the stride-1 3x3 convs in F8 mode, 8 x 16 tiles (p.Wt, p.Ht), k-blocks in the
+// order channel chunk, dx, dy, over the whole K range.
+template <int BN, bool RES, bool F8, bool VQ = false, int EXT = 0, bool COLS = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                 const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const TcP p) {
-  using Cfg = TcCfg<BN>;
-  constexpr int STAGES = Cfg::STAGES, NF = Cfg::NF;
+  using Cfg = TcCfg<BN, COLS>;
+  constexpr int STAGES = Cfg::STAGES, COL_STAGES = Cfg::COL_STAGES, NF = Cfg::NF;
   static_assert(!VQ || (!RES && !F8), "VQ mode: plain linear tiles");
+  static_assert(!COLS || (F8 && !VQ && EXT == 0), "column schedule: F8 3x3 convs");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
+  const uint32_t ring_base = smem_base + Cfg::COL_RING_BYTES;      // the stage ring
+  const uint32_t bar_base = smem_base + Cfg::RING_BYTES;
   float* red = reinterpret_cast<float*>(smem_raw + (bar_base + 256u - smem_u32(smem_raw)));
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  auto col_full_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
+  auto col_empty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + COL_STAGES + s); };
 
   const int worker = (int)blockIdx.x, nworkers = (int)gridDim.x;
   const int num_m = p.num_tiles / p.n_tiles;
@@ -258,6 +278,7 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
   pdl_launch_dependents();        // the next kernel of the stream may begin its own prologue as our CTAs retire
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TC_CONSUMER_WARPS); }
+    for (int s = 0; s < COL_STAGES; ++s) { mbar_init(col_full_bar(s), 1); mbar_init(col_empty_bar(s), TC_CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -266,6 +287,34 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
   if (warp == TC_CONSUMER_WARPS) {
     // ===================== TMA producer =====================
     if (!elect_one()) return;
+    if constexpr (COLS) {
+      // per (chunk, dx): the column box at (x + dx, y - 1), then the weight boxes of taps (-1, dx), (0, dx), (+1, dx)
+      int stage = 0, cstage = 0; uint32_t phase = 0, cphase = 0;
+      for (int it = 0, work; (work = work_of(it)) >= 0; ++it) {
+        const TileCoord tc = decode(work);
+        const int n0 = tc.nt * BN, x0 = tc.tx * COL_WT, y0 = tc.ty * COL_HT - 1;
+        for (int c0 = 0; c0 < p.Cin; c0 += TC_BK) {
+          for (int dx = 0; dx < 3; ++dx) {
+            mbar_wait(col_empty_bar(cstage), cphase ^ 1u);
+            const uint32_t ca = smem_base + cstage * COL_STAGE_BYTES;
+            mbar_expect_tx(col_full_bar(cstage), COL_STAGE_BYTES);
+            tma_load_4d(ca, &map_a_hi, col_full_bar(cstage), c0, x0 + dx - 1, y0, tc.b);
+            tma_load_4d(ca + COL_PLANE_BYTES, &map_a_lo, col_full_bar(cstage), c0, x0 + dx - 1, y0, tc.b);
+            if (++cstage == COL_STAGES) { cstage = 0; cphase ^= 1u; }
+            for (int dy = 0; dy < 3; ++dy) {
+              const int k0 = (3 * dy + dx) * p.Cin + c0;
+              mbar_wait(empty_bar(stage), phase ^ 1u);
+              const uint32_t sb = ring_base + stage * Cfg::STAGE_BYTES;
+              mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
+              tma_load_2d(sb, &map_b_hi, full_bar(stage), k0, n0);
+              tma_load_2d(sb + Cfg::B_PLANE_BYTES, &map_b_lo, full_bar(stage), k0, n0);
+              if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+            }
+          }
+        }
+      }
+      return;
+    }
     const int ksz = EXT == 1 && p.taps == 16 ? 4 : EXT == 2 && p.taps == 25 ? 5 : (p.taps == 9 ? 3 : 1);   // (p.up: taps == 4)
     int stage = 0; uint32_t phase = 0;
     for (int it = 0, work; (work = work_of(it)) >= 0; ++it) {
@@ -306,6 +355,7 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
 #pragma unroll
   for (int i = 0; i < NF; ++i) { acc[i] = 0.f; ext[i] = 0.f; }
   int stage = 0; uint32_t phase = 0;
+  uint32_t ncol = 0;                     // COLS: column boxes consumed (the column ring's position)
   // VQ state: the running top-4 of this thread's two rows
   float td[2][4];
   int tj[2][4];
@@ -315,42 +365,78 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
     const TileCoord tc = decode(work);
     // ---------------- main loop
     bool have_ext = F8;
-    for (int kb0 = p.kb_begin; kb0 < p.kb_end; kb0 += slice_len) {
-      const int kb1 = min(kb0 + slice_len, p.kb_end);
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(full_bar(stage), phase);
-        const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-        const uint64_t a_hi = make_sw128_desc(sa + wg * (A_PLANE_BYTES / 2));
-        const uint64_t a_lo = make_sw128_desc(sa + A_PLANE_BYTES + wg * (A_PLANE_BYTES / 2));
-        const uint64_t b_hi = make_sw128_desc(sa + 2 * A_PLANE_BYTES);
-        const uint64_t b_lo = make_sw128_desc(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES);
-        fence_regs(acc); fence_regs(ext);
-        wgmma_fence();
+    if constexpr (COLS) {
+      // same wgmmas per k-block as below (e4m3 cross term, then hi * hi); the A operand of tap dy starts 8 (dy + 1)
+      // rows into the column box, and the box is released after its third tap
+      uint32_t more = 0;
+      for (int col = 0; col < 3 * p.cchunks; ++col, ++ncol) {        // (chunk, dx) in that order
+        const int cs = ncol % COL_STAGES;
+        mbar_wait(col_full_bar(cs), (ncol / COL_STAGES) & 1u);
+        const uint32_t ca = smem_base + cs * COL_STAGE_BYTES + wg * (A_PLANE_BYTES / 2);
+#pragma unroll 1
+        for (int dy = 0; dy < 3; ++dy) {
+          mbar_wait(full_bar(stage), phase);
+          const uint32_t sb = ring_base + stage * Cfg::STAGE_BYTES;
+          const uint64_t a_hi = make_sw128_desc(ca + 1024 * dy);
+          const uint64_t a_lo = make_sw128_desc(ca + COL_PLANE_BYTES + 1024 * dy);
+          const uint64_t b_hi = make_sw128_desc(sb);
+          const uint64_t b_lo = make_sw128_desc(sb + Cfg::B_PLANE_BYTES);
+          fence_regs(acc); fence_regs(ext);
+          wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k) {
-          const uint64_t ko = (uint64_t)((k * 32) >> 4);   // +32 bytes per k-step inside the 128B swizzle atom
-          const uint32_t more = (kb != kb0 || k != 0) ? 1u : 0u;
-          // small cross terms first, the dominant hi*hi product last
-          if constexpr (F8) {
-            Wgmma<BN>::e4m3(ext, a_lo + ko, b_lo + ko, more);     // sum a_lo8 w_hi8 + sum a_hi8 w_lo8
-            Wgmma<BN>::f16(acc, a_hi + ko, b_hi + ko, more);
-          } else {
-            Wgmma<BN>::f16(acc, a_lo + ko, b_hi + ko, more);
-            Wgmma<BN>::f16(acc, a_hi + ko, b_lo + ko, 1u);
-            Wgmma<BN>::f16(acc, a_hi + ko, b_hi + ko, 1u);
+          for (int k = 0; k < TC_BK / 16; ++k) {
+            const uint64_t ko = (uint64_t)((k * 32) >> 4);
+            Wgmma<BN>::e4m3(ext, a_lo + ko, b_lo + ko, k ? 1u : more);
+            Wgmma<BN>::f16(acc, a_hi + ko, b_hi + ko, k ? 1u : more);
           }
+          wgmma_commit();
+          wgmma_wait_all();
+          fence_regs(acc); fence_regs(ext);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(stage));
+          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+          more = 1u;
         }
-        wgmma_commit();
-        wgmma_wait_all();
-        fence_regs(acc); fence_regs(ext);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar(stage));     // this warp's reads of the stage are complete
-        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+        if (lane == 0) mbar_arrive(col_empty_bar(cs));
       }
-      if (kb1 < p.kb_end) {           // sliced: fold the finished partial into the running sum
+    } else {
+      for (int kb0 = p.kb_begin; kb0 < p.kb_end; kb0 += slice_len) {
+        const int kb1 = min(kb0 + slice_len, p.kb_end);
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(full_bar(stage), phase);
+          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
+          const uint64_t a_hi = make_sw128_desc(sa + wg * (A_PLANE_BYTES / 2));
+          const uint64_t a_lo = make_sw128_desc(sa + A_PLANE_BYTES + wg * (A_PLANE_BYTES / 2));
+          const uint64_t b_hi = make_sw128_desc(sa + 2 * A_PLANE_BYTES);
+          const uint64_t b_lo = make_sw128_desc(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES);
+          fence_regs(acc); fence_regs(ext);
+          wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < NF; ++i) ext[i] = have_ext ? acc[i] + ext[i] : acc[i];
-        have_ext = true;
+          for (int k = 0; k < TC_BK / 16; ++k) {
+            const uint64_t ko = (uint64_t)((k * 32) >> 4);   // +32 bytes per k-step inside the 128B swizzle atom
+            const uint32_t more = (kb != kb0 || k != 0) ? 1u : 0u;
+            // small cross terms first, the dominant hi*hi product last
+            if constexpr (F8) {
+              Wgmma<BN>::e4m3(ext, a_lo + ko, b_lo + ko, more);     // sum a_lo8 w_hi8 + sum a_hi8 w_lo8
+              Wgmma<BN>::f16(acc, a_hi + ko, b_hi + ko, more);
+            } else {
+              Wgmma<BN>::f16(acc, a_lo + ko, b_hi + ko, more);
+              Wgmma<BN>::f16(acc, a_hi + ko, b_lo + ko, 1u);
+              Wgmma<BN>::f16(acc, a_hi + ko, b_hi + ko, 1u);
+            }
+          }
+          wgmma_commit();
+          wgmma_wait_all();
+          fence_regs(acc); fence_regs(ext);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(stage));     // this warp's reads of the stage are complete
+          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+        }
+        if (kb1 < p.kb_end) {           // sliced: fold the finished partial into the running sum
+#pragma unroll
+          for (int i = 0; i < NF; ++i) ext[i] = have_ext ? acc[i] + ext[i] : acc[i];
+          have_ext = true;
+        }
       }
     }
     if (have_ext) {
@@ -867,24 +953,26 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
-template <int BN, bool RES, bool F8, bool VQ, int EXT = 0>
+template <int BN, bool RES, bool F8, bool VQ, int EXT = 0, bool COLS = false>
 static int launch_tc_v(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
                        const TcP& p, cudaStream_t st) {
-  using Cfg = TcCfg<BN>;
+  using Cfg = TcCfg<BN, COLS>;
   static PerDeviceFlag attr_set;      // per template instantiation AND per device
   if (!attr_set.cur()) {
-    FEMASR_CUDA(cudaFuncSetAttribute(tc_igemm_kernel<BN, RES, F8, VQ, EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    FEMASR_CUDA(cudaFuncSetAttribute(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set.cur() = true;
   }
   const int items = VQ ? p.num_tiles / p.n_tiles : p.num_tiles;     // VQ: one CTA walks all code tiles of an m-tile
   const int grid = items < sm_count() ? items : sm_count();
-  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ, EXT>, dim3(grid), dim3(TC_THREADS), Cfg::SMEM_BYTES, st, ah, al, bh, bl, p));
+  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS>, dim3(grid), dim3(TC_THREADS), Cfg::SMEM_BYTES, st, ah, al, bh, bl, p));
   return launch_status(VQ ? "tc_igemm_kernel(vq)" : "tc_igemm_kernel");
 }
 
 template <int BN>
 static int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
-                     const TcP& p, cudaStream_t st) {
+                     const TcP& p, bool cols, cudaStream_t st) {
+  if (cols)
+    return p.res1 ? launch_tc_v<BN, true, true, false, 0, true>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, true, false, 0, true>(ah, al, bh, bl, p, st);
   if (p.f8) return p.res1 ? launch_tc_v<BN, true, true, false>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, true, false>(ah, al, bh, bl, p, st);
   if (p.taps == 25)
     return p.res1 ? launch_tc_v<BN, true, false, false, 2>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false, 2>(ah, al, bh, bl, p, st);
@@ -911,13 +999,22 @@ static void tc_tile_shape(int H, int W, int* Wt, int* Ht) {
 // 128-wide tiles where Cout allows (a 128 x 128 fp32 accumulator is 64 registers per consumer thread, which leaves room
 // for the F8 cross-product / K-slice accumulator beside it), else 64-wide.  femasr_tc_args.pair / .strip select
 // schedules of other GPU generations and do not change the tiling here.
-struct TilePlan { int Wt, Ht, wt_shift, tiles_x, tiles_y, BN; };
+// The stride-1 3x3 convs in F8 mode over the whole K range run the column schedule (8 x 16 tiles, TcCfg) wherever it
+// needs no more tiles than tc_tile_shape's choice: every map behind the VQ, whose sides are multiples of 16.  The tile
+// count, and with it the GroupNorm partial-row count, is then the same for both schedules.  FEMASR_TC_COLUMNS=0 keeps
+// the tap-order schedule (for A/B timing).
+struct TilePlan { int Wt, Ht, wt_shift, tiles_x, tiles_y, BN; bool cols; };
 static TilePlan plan_tiles(const femasr_tc_args* a, int H, int W) {
+  static const int cols_env = [] { const char* e = getenv("FEMASR_TC_COLUMNS"); return e ? atoi(e) : 1; }();
   TilePlan t;
   t.BN = a->Cout % 128 == 0 ? 128 : 64;
   tc_tile_shape(H, W, &t.Wt, &t.Ht);   // the widest power-of-two Wt <= 128 that wastes the fewest padded pixels
-  t.wt_shift = 0; while ((1 << t.wt_shift) < t.Wt) ++t.wt_shift;
   t.tiles_x = (int)cdiv(W, t.Wt); t.tiles_y = (int)cdiv(H, t.Ht);
+  const long nkb = 9l * (a->Cin / 64);
+  t.cols = cols_env && a->f8 && a->ksize == 3 && a->stride != 2 && !a->upsample && a->kb_begin == 0 &&
+           (a->kb_count == 0 || a->kb_count == nkb) && cdiv(W, COL_WT) * cdiv(H, COL_HT) == (long)t.tiles_x * t.tiles_y;
+  if (t.cols) { t.Wt = COL_WT; t.Ht = COL_HT; t.tiles_x = (int)cdiv(W, COL_WT); t.tiles_y = (int)cdiv(H, COL_HT); }
+  t.wt_shift = 0; while ((1 << t.wt_shift) < t.Wt) ++t.wt_shift;
   return t;
 }
 
@@ -1175,7 +1272,8 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
     const cuuint64_t dims[4] = {(cuuint64_t)a->Cin, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B};
     const cuuint64_t str[3] = {(cuuint64_t)a->Cin * 2, (cuuint64_t)Win * a->Cin * 2, (cuuint64_t)Hin * Win * a->Cin * 2};
     // with a traversal stride s the box spans s*Wt x s*Ht source pixels and lands Wt x Ht of them in smem
-    const cuuint32_t box[4] = {64, (cuuint32_t)(p.Wt * stride), (cuuint32_t)(p.Ht * stride), 1};
+    // column schedule: the box spans the tile's 16 rows plus the rows above and below
+    const cuuint32_t box[4] = {64, (cuuint32_t)(p.Wt * stride), (cuuint32_t)(plan.cols ? COL_HT + 2 : p.Ht * stride), 1};
     int s = make_map(&mah, a->a_hi, 4, dims, str, box, stride);
     if (s) return s;
     s = make_map(&mal, a->a_lo, 4, dims, str, box, stride);
@@ -1191,6 +1289,6 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
     if (s) return s;
   }
   cudaStream_t st = as_stream(stream);
-  if (BN == 128) return launch_tc<128>(mah, mal, mbh, mbl, p, st);
-  return launch_tc<64>(mah, mal, mbh, mbl, p, st);
+  if (BN == 128) return launch_tc<128>(mah, mal, mbh, mbl, p, plan.cols, st);
+  return launch_tc<64>(mah, mal, mbh, mbl, p, plan.cols, st);
 }

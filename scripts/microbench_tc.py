@@ -1,7 +1,16 @@
 """Per-shape timing of the tensor-core implicit GEMM through the C ABI (CUDA events, L2 flushed between reps).
 Usage (GPU box): python scripts/microbench_tc.py > gpurun_out/microbench.txt"""
 import os
+import subprocess
 import sys
+
+# MB_COLUMNS=ab: the F8 3x3 cases twice, on the column schedule (FEMASR_TC_COLUMNS=1) and on the tap-order one (=0)
+if os.environ.get('MB_COLUMNS') == 'ab':
+    for v in ('1', '0'):
+        print(f"# FEMASR_TC_COLUMNS={v}", flush=True)
+        env = dict(os.environ, MB_COLUMNS='', MB_F8='1', MB_ONLY=os.environ.get('MB_ONLY') or 'conv', FEMASR_TC_COLUMNS=v)
+        subprocess.run([sys.executable, os.path.abspath(__file__)], env=env, check=True)
+    sys.exit(0)
 
 import torch
 
