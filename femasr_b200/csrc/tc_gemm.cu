@@ -15,6 +15,8 @@
 //   warps 0-7  two consumer warpgroups, each owning 64 rows of the 128 x BN tile: wgmma m64nBNk16 straight from the
 //              swizzled shared-memory stages into a register accumulator, then the epilogue from those registers
 //              (*2^-s + bias -> GELU -> + residual(s) -> fp32 NHWC or split-fp16 planes, GroupNorm partials, VQ top-4).
+// The ping-pong schedule (PP, 384 threads) gives the producer a warpgroup of its own and each consumer warpgroup whole
+// tiles, in turns on the tensor cores, so that one tile's epilogue runs under the next tile's MMAs.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
@@ -99,6 +101,13 @@ __device__ __forceinline__ bool elect_one() {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+
+// Named barriers of the ping-pong schedule, and the per-warpgroup register budgets (setmaxnreg, one whole warpgroup)
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 // m64nNk16 (f16) / m64nNk32 (e4m3) with N / 2 fp32 accumulator registers per thread; operands after them: A and B
 // descriptors, then the accumulate flag
 #define FEMASR_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
@@ -181,6 +190,11 @@ struct TcP {
 constexpr int TC_BM = 128, TC_BK = 64;
 constexpr int A_PLANE_BYTES = TC_BM * TC_BK * 2;   // 16 KB
 constexpr int TC_CONSUMER_WARPS = 8, TC_THREADS = 32 * TC_CONSUMER_WARPS + 32;
+// Ping-pong schedule (PP): a whole producer warpgroup, so that setmaxnreg (which acts on warpgroups) can move its
+// registers to the consumers: 128 x 40 + 256 x 232 = 64512 <= 65536, the 168 per thread of the launch.
+constexpr int TC_PP_THREADS = 32 * TC_CONSUMER_WARPS + 128;
+constexpr int PP_PRODUCER_REGS = 40, PP_CONSUMER_REGS = 232;
+constexpr int PP_GN_BAR = 2, PP_ORDER_BAR = 4;     // named barriers (+ warpgroup); 1 is the cooperative epilogue's
 constexpr int TC_SMEM_LIMIT = 232448;              // 227 KB of opt-in shared memory per block on H100
 
 // Column schedule (COLS): 8 x 16 output tiles; one activation box of 64 ch x 8 cols x 18 rows per (channel chunk, dx)
@@ -221,6 +235,96 @@ __device__ __forceinline__ void top4_insert(float (&td)[4], int (&tj)[4], float 
     }
 }
 
+// Epilogue of one warp's 16 accumulator rows of a tile (rows row0 + lane / 4 and row0 + lane / 4 + 8):
+// acc * 2^-s + bias -> GELU | ReLU -> + res1 + res2 -> store.  With GroupNorm partials, the warp's per-group sum and sum
+// of squares over its 16 rows go to red_row[2 g], red_row[2 g + 1].  Used by the ping-pong schedule (BN 64).  The
+// cooperative schedule keeps its inline copy, which loads each residual inside the store loop: calling this helper there
+// changes ptxas's allocation in every cooperative instantiation, and at BN 128 the residual registers spill.  Both copies
+// compute the same values (tests/test_tc_pingpong_gpu.py compares bytes).
+template <int BN, bool RES, int EXT, class TileCoord>
+__device__ __forceinline__ void epilogue_rows(const TcP& p, const TileCoord& tc, const float (&acc)[BN / 2], int row0,
+                                              float inv_scale, float* red_row, int lane) {
+  const int rsub = lane >> 2, q = lane & 3;
+  const int Ho = p.up ? 2 * p.H : p.H, Wo = p.up ? 2 * p.W : p.W;
+  long off[2];                                         // output element offset of this thread's two rows (-1: outside)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + rsub + 8 * h;
+    const int y = tc.ty * p.Ht + (row >> p.wt_shift), x = tc.tx * p.Wt + (row & (p.Wt - 1));
+    const int oy = p.up ? 2 * y + (tc.ph >> 1) : y, ox = p.up ? 2 * x + (tc.ph & 1) : x;
+    off[h] = (y < p.H && x < p.W) ? (((long)tc.b * Ho + oy) * Wo + ox) * p.Cout : -1;
+  }
+  // The thread's residuals are all loaded before its first store.  As far as the compiler knows the stores may alias
+  // res1 (they do in the in-place residual convs), so a load issued inside the store loop would wait for the previous
+  // stores and pay one memory round trip per column block and row.  Each element is still read before its own store.
+  float2 r1[RES ? BN / 8 : 1][2];
+  if constexpr (RES) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        r1[j][h] = off[h] >= 0 ? *reinterpret_cast<const float2*>(p.res1 + off[h] + tc.nt * BN + 8 * j + 2 * q)
+                               : make_float2(0.f, 0.f);
+  }
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = tc.nt * BN + 8 * j + 2 * q;
+    const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
+    float gs = 0.f, gss = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float2 o;
+      o.x = fmaf(acc[4 * j + 2 * h], inv_scale, bb.x);     // acc * 2^-s is exact: == (acc * inv) + bias
+      o.y = fmaf(acc[4 * j + 2 * h + 1], inv_scale, bb.y);
+      if (p.act == FEMASR_ACT_GELU) { o.x = gelu_erf_fast_f(o.x); o.y = gelu_erf_fast_f(o.y); }
+      else if (p.act == FEMASR_ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+      else if (EXT == 1 && p.act == FEMASR_ACT_LRELU) { o.x = lrelu02_f(o.x); o.y = lrelu02_f(o.y); }
+      if (off[h] >= 0) {
+        const long o_off = off[h] + col;
+        if (RES) { o.x += r1[j][h].x; o.y += r1[j][h].y; }
+        if (p.res2) { const float2 r = *reinterpret_cast<const float2*>(p.res2 + o_off); o.x += r.x; o.y += r.y; }
+        if (p.out_hi) {
+          uint32_t hh, ll;
+          split_pack2(o.x, o.y, hh, ll);
+          *reinterpret_cast<uint32_t*>(p.out_hi + o_off) = hh;
+          *reinterpret_cast<uint32_t*>(p.out_lo + o_off) = ll;
+        } else {
+          *reinterpret_cast<float2*>(p.y + o_off) = o;
+        }
+        gs += o.x + o.y; gss = fmaf(o.x, o.x, fmaf(o.y, o.y, gss));
+      }
+    }
+    if (p.gn_partial) {
+      // fixed-order reduction over the warp's 16 rows (lanes sharing q), then over the lanes of one group
+#pragma unroll
+      for (int o = 4; o <= 16; o <<= 1) { gs += __shfl_xor_sync(0xffffffffu, gs, o); gss += __shfl_xor_sync(0xffffffffu, gss, o); }
+      if (p.cpg >= 4) { gs += __shfl_xor_sync(0xffffffffu, gs, 1); gss += __shfl_xor_sync(0xffffffffu, gss, 1); }
+      if (p.cpg >= 8) { gs += __shfl_xor_sync(0xffffffffu, gs, 2); gss += __shfl_xor_sync(0xffffffffu, gss, 2); }
+      if (rsub == 0 && (q & (p.cpg / 2 - 1)) == 0) {
+        const int g = (8 * j + 2 * q) / p.cpg;
+        red_row[g * 2] = gs;
+        red_row[g * 2 + 1] = gss;
+      }
+    }
+  }
+}
+
+// One GroupNorm partial row per 32-row quarter of the tile: the sum of the two 16-row warp partials that cover it, in
+// that order.  red holds the warp partials of 16-row group k at red[2 (k * gslots + g)]; threads tid = 0 .. nthreads - 1.
+template <int BN, class TileCoord>
+__device__ __forceinline__ void gn_store_partials(const TcP& p, const TileCoord& tc, const float* red, int gslots, int tid,
+                                                  int nthreads) {
+  const int gpl = BN / p.cpg;                           // GroupNorm groups of this n-tile
+  const int tile_in_img = (tc.ph * p.tiles_y + tc.ty) * p.tiles_x + tc.tx;
+  for (int i = tid; i < 4 * gpl; i += nthreads) {
+    const int quarter = i / gpl, g = i - quarter * gpl;
+    const float* r0 = red + ((2 * quarter) * gslots + g) * 2;
+    const float* r1 = red + ((2 * quarter + 1) * gslots + g) * 2;
+    float* gp = p.gn_partial + (((long)tc.b * p.gn_rows + tile_in_img * 4 + quarter) * 32 + tc.nt * gpl + g) * 2;
+    *reinterpret_cast<float2*>(gp) = make_float2(r0[0] + r1[0], r0[1] + r1[1]);
+  }
+}
+
 // RES: the layer adds a residual tile (res1) in the epilogue (a template parameter: the load is in the hot loop).
 // F8: the F8 cross-term mode (p.f8).  A template parameter because a runtime choice between the two accumulator sets
 // inside the k-loop makes ptxas serialise every wgmma of the kernel.
@@ -231,14 +335,17 @@ __device__ __forceinline__ void top4_insert(float (&td)[4], int (&tj)[4], float 
 // stream they had without them (measured: 1.3% slower GEMMs otherwise).
 // COLS: the column schedule (TcCfg) of the stride-1 3x3 convs in F8 mode, 8 x 16 tiles (p.Wt, p.Ht), k-blocks in the
 // order channel chunk, dx, dy, over the whole K range.
-template <int BN, bool RES, bool F8, bool VQ = false, int EXT = 0, bool COLS = false>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+// PP: the ping-pong schedule (TC_PP_THREADS) of the BN-64 launches: each consumer warpgroup owns whole 128-row tiles,
+// the two take turns on the tensor cores, and one runs its epilogue while the other runs its k-loop (plan_tiles).
+template <int BN, bool RES, bool F8, bool VQ = false, int EXT = 0, bool COLS = false, bool PP = false>
+__global__ void __launch_bounds__(PP ? TC_PP_THREADS : TC_THREADS, 1)
 tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                 const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const TcP p) {
   using Cfg = TcCfg<BN, COLS>;
   constexpr int STAGES = Cfg::STAGES, COL_STAGES = Cfg::COL_STAGES, NF = Cfg::NF;
   static_assert(!VQ || (!RES && !F8), "VQ mode: plain linear tiles");
   static_assert(!COLS || (F8 && !VQ && EXT == 0), "column schedule: F8 3x3 convs");
+  static_assert(!PP || (BN == 64 && !VQ), "ping-pong schedule: BN-64 convs and linears");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t ring_base = smem_base + Cfg::COL_RING_BYTES;      // the stage ring
@@ -277,15 +384,21 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   pdl_launch_dependents();        // the next kernel of the stream may begin its own prologue as our CTAs retire
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TC_CONSUMER_WARPS); }
-    for (int s = 0; s < COL_STAGES; ++s) { mbar_init(col_full_bar(s), 1); mbar_init(col_empty_bar(s), TC_CONSUMER_WARPS); }
+    // a stage (column box) is released by every warp that reads it: all consumer warps, or (PP) one warpgroup's
+    constexpr int READERS = PP ? TC_CONSUMER_WARPS / 2 : TC_CONSUMER_WARPS;
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), READERS); }
+    for (int s = 0; s < COL_STAGES; ++s) { mbar_init(col_full_bar(s), 1); mbar_init(col_empty_bar(s), READERS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   pdl_wait();                     // barriers initialised: from here on the predecessor's output is read
 
-  if (warp == TC_CONSUMER_WARPS) {
+  if (PP ? warp >= TC_CONSUMER_WARPS : warp == TC_CONSUMER_WARPS) {
     // ===================== TMA producer =====================
+    if constexpr (PP) {
+      setmaxnreg_dec<PP_PRODUCER_REGS>();      // the whole warpgroup; one lane of its first warp issues the loads
+      if (warp != TC_CONSUMER_WARPS) return;
+    }
     if (!elect_one()) return;
     if constexpr (COLS) {
       // per (chunk, dx): the column box at (x + dx, y - 1), then the weight boxes of taps (-1, dx), (0, dx), (+1, dx)
@@ -338,6 +451,118 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
         tma_load_2d(sa + 2 * A_PLANE_BYTES, &map_b_hi, full_bar(stage), tap * p.Cin + c0, n0);
         tma_load_2d(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES, &map_b_lo, full_bar(stage), tap * p.Cin + c0, n0);
         if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+      }
+    }
+    return;
+  }
+
+  if constexpr (PP) {
+    // ===================== ping-pong consumers: warpgroup wg takes work items it = wg, wg + 2, ... =====================
+    // Both halves of the tile (rows 0-63, 64-127) are m64 accumulators of the same warpgroup, each summed in the same
+    // product order as in the cooperative schedule.  The producer fills the rings in work-item order and every item has
+    // the same number of k-blocks, so a warpgroup finds its ring positions by skipping the other's items.  An order
+    // barrier (PP_ORDER_BAR + wg) hands the tensor cores over at the end of each k-loop: the other warpgroup's k-loop
+    // then overlaps this one's epilogue.
+    setmaxnreg_inc<PP_CONSUMER_REGS>();
+    const int wg = warp >> 2;
+    const float inv_scale = __ldg(p.inv_scale);
+    const int nkb = COLS ? 9 * p.cchunks : p.kb_end - p.kb_begin;   // k-blocks per work item
+    int stage = 0; uint32_t phase = 0;
+    uint32_t ncol = 0;                     // COLS: column boxes consumed (the column ring's position)
+    auto skip_item = [&]() {
+      stage += nkb;
+      while (stage >= STAGES) { stage -= STAGES; phase ^= 1u; }
+      if (COLS) ncol += 3 * p.cchunks;
+    };
+    if (wg == 1) skip_item();
+    float* red_wg = red + wg * 8 * 32 * 2;   // 8 groups of 16 rows x at most 32 GroupNorm groups per warpgroup
+    for (int it = wg, work; (work = work_of(it)) >= 0; it += 2) {
+      const TileCoord tc = decode(work);
+      float acc[2][NF], ext[2][NF];
+      if (it > 0) named_bar_sync(PP_ORDER_BAR + wg, 256);     // the previous item's k-loop is issued
+      // One k-block of wgmmas stays in flight: a stage (and a column box after its third tap) is released once the
+      // next k-block's wgmma.wait_group 1 has returned.
+      int rel_stage = -1, rel_col = -1;
+      auto release = [&]() {
+        __syncwarp();
+        if (lane == 0) {
+          if (rel_stage >= 0) mbar_arrive(empty_bar(rel_stage));
+          if (rel_col >= 0) mbar_arrive(col_empty_bar(rel_col));
+        }
+      };
+      auto kblock = [&](uint32_t a0, uint32_t a1, uint32_t b_addr, uint32_t more) {
+        const uint64_t b_hi = make_sw128_desc(b_addr);
+        const uint64_t b_lo = make_sw128_desc(b_addr + Cfg::B_PLANE_BYTES);
+        fence_regs(acc[0]); fence_regs(acc[1]);
+        if (F8) { fence_regs(ext[0]); fence_regs(ext[1]); }
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k) {
+          const uint64_t ko = (uint64_t)((k * 32) >> 4);
+          const uint32_t m = k ? 1u : more;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint64_t a_hi = make_sw128_desc(a0 + h * (A_PLANE_BYTES / 2));
+            const uint64_t a_lo = make_sw128_desc(a1 + h * (A_PLANE_BYTES / 2));
+            if constexpr (F8) {
+              Wgmma<BN>::e4m3(ext[h], a_lo + ko, b_lo + ko, m);
+              Wgmma<BN>::f16(acc[h], a_hi + ko, b_hi + ko, m);
+            } else {
+              Wgmma<BN>::f16(acc[h], a_lo + ko, b_hi + ko, m);
+              Wgmma<BN>::f16(acc[h], a_hi + ko, b_lo + ko, 1u);
+              Wgmma<BN>::f16(acc[h], a_hi + ko, b_hi + ko, 1u);
+            }
+          }
+        }
+        wgmma_commit();
+        wgmma_wait_1();
+        fence_regs(acc[0]); fence_regs(acc[1]);
+        if (F8) { fence_regs(ext[0]); fence_regs(ext[1]); }
+        release();
+      };
+      if constexpr (COLS) {
+        for (int col = 0; col < 3 * p.cchunks; ++col, ++ncol) {        // (chunk, dx) in that order
+          const int cs = ncol % COL_STAGES;
+          mbar_wait(col_full_bar(cs), (ncol / COL_STAGES) & 1u);
+          const uint32_t ca = smem_base + cs * COL_STAGE_BYTES;
+#pragma unroll 1
+          for (int dy = 0; dy < 3; ++dy) {
+            mbar_wait(full_bar(stage), phase);
+            kblock(ca + 1024 * dy, ca + COL_PLANE_BYTES + 1024 * dy, ring_base + stage * Cfg::STAGE_BYTES, col || dy ? 1u : 0u);
+            rel_stage = stage; rel_col = dy == 2 ? cs : -1;
+            if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+          }
+        }
+      } else {
+        for (int kb = p.kb_begin; kb < p.kb_end; ++kb) {
+          mbar_wait(full_bar(stage), phase);
+          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
+          kblock(sa, sa + A_PLANE_BYTES, sa + 2 * A_PLANE_BYTES, kb != p.kb_begin ? 1u : 0u);
+          rel_stage = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+        }
+      }
+      if (work_of(it + 1) >= 0) named_bar_arrive(PP_ORDER_BAR + (wg ^ 1), 256);
+      wgmma_wait_all();
+      fence_regs(acc[0]); fence_regs(acc[1]);
+      if (F8) { fence_regs(ext[0]); fence_regs(ext[1]); }
+      release();
+      skip_item();                                       // the other warpgroup's next item
+      if (F8) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int i = 0; i < NF; ++i) acc[h][i] += ext[h][i];
+      }
+      // 16-row group 4 h + warp % 4 of the tile: the same rows, shuffles and GroupNorm sums as warp 4 h + warp % 4 of
+      // the cooperative schedule
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        epilogue_rows<BN, RES, EXT>(p, tc, acc[h], h * 64 + (warp & 3) * 16, inv_scale, red_wg + (4 * h + (warp & 3)) * 32 * 2, lane);
+      if (p.gn_partial) {
+        named_bar_sync(PP_GN_BAR + wg, 128);
+        gn_store_partials<BN>(p, tc, red_wg, 32, threadIdx.x & 127, 128);
+        named_bar_sync(PP_GN_BAR + wg, 128);
       }
     }
     return;
@@ -953,32 +1178,33 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
-template <int BN, bool RES, bool F8, bool VQ, int EXT = 0, bool COLS = false>
+template <int BN, bool RES, bool F8, bool VQ, int EXT = 0, bool COLS = false, bool PP = false>
 static int launch_tc_v(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
                        const TcP& p, cudaStream_t st) {
   using Cfg = TcCfg<BN, COLS>;
   static PerDeviceFlag attr_set;      // per template instantiation AND per device
   if (!attr_set.cur()) {
-    FEMASR_CUDA(cudaFuncSetAttribute(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    FEMASR_CUDA(cudaFuncSetAttribute(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set.cur() = true;
   }
   const int items = VQ ? p.num_tiles / p.n_tiles : p.num_tiles;     // VQ: one CTA walks all code tiles of an m-tile
   const int grid = items < sm_count() ? items : sm_count();
-  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS>, dim3(grid), dim3(TC_THREADS), Cfg::SMEM_BYTES, st, ah, al, bh, bl, p));
+  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP>, dim3(grid), dim3(PP ? TC_PP_THREADS : TC_THREADS), Cfg::SMEM_BYTES, st, ah, al, bh, bl, p));
   return launch_status(VQ ? "tc_igemm_kernel(vq)" : "tc_igemm_kernel");
 }
 
-template <int BN>
+// PP: the ping-pong schedule (plan_tiles decides)
+template <int BN, bool PP = false>
 static int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
                      const TcP& p, bool cols, cudaStream_t st) {
   if (cols)
-    return p.res1 ? launch_tc_v<BN, true, true, false, 0, true>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, true, false, 0, true>(ah, al, bh, bl, p, st);
-  if (p.f8) return p.res1 ? launch_tc_v<BN, true, true, false>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, true, false>(ah, al, bh, bl, p, st);
+    return p.res1 ? launch_tc_v<BN, true, true, false, 0, true, PP>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, true, false, 0, true, PP>(ah, al, bh, bl, p, st);
+  if (p.f8) return p.res1 ? launch_tc_v<BN, true, true, false, 0, false, PP>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, true, false, 0, false, PP>(ah, al, bh, bl, p, st);
   if (p.taps == 25)
-    return p.res1 ? launch_tc_v<BN, true, false, false, 2>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false, 2>(ah, al, bh, bl, p, st);
+    return p.res1 ? launch_tc_v<BN, true, false, false, 2, false, PP>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false, 2, false, PP>(ah, al, bh, bl, p, st);
   if (p.taps == 16 || p.act == FEMASR_ACT_LRELU)
-    return p.res1 ? launch_tc_v<BN, true, false, false, 1>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false, 1>(ah, al, bh, bl, p, st);
-  return p.res1 ? launch_tc_v<BN, true, false, false>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false>(ah, al, bh, bl, p, st);
+    return p.res1 ? launch_tc_v<BN, true, false, false, 1, false, PP>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false, 1, false, PP>(ah, al, bh, bl, p, st);
+  return p.res1 ? launch_tc_v<BN, true, false, false, 0, false, PP>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false, 0, false, PP>(ah, al, bh, bl, p, st);
 }
 
 }  // namespace femasr
@@ -1003,9 +1229,15 @@ static void tc_tile_shape(int H, int W, int* Wt, int* Ht) {
 // needs no more tiles than tc_tile_shape's choice: every map behind the VQ, whose sides are multiples of 16.  The tile
 // count, and with it the GroupNorm partial-row count, is then the same for both schedules.  FEMASR_TC_COLUMNS=0 keeps
 // the tap-order schedule (for A/B timing).
-struct TilePlan { int Wt, Ht, wt_shift, tiles_x, tiles_y, BN; bool cols; };
-static TilePlan plan_tiles(const femasr_tc_args* a, int H, int W) {
+// The ping-pong schedule (tc_igemm_kernel's PP) runs the BN-64 launches that are not K-sliced (`sliced`: the launch's
+// effective slicing); a warpgroup holds a whole 128 x 64 tile, F8 accumulator included.  BN 128 keeps the cooperative
+// schedule: with F8 or K slicing its two accumulators do not fit in one warpgroup, and without them (the linears)
+// ping-pong measured slower on H100 - their short k-loops cannot hide an epilogue that one warpgroup runs alone.  It
+// changes neither the tiling nor any sum.  FEMASR_TC_PINGPONG=0 keeps the cooperative schedule (for A/B timing).
+struct TilePlan { int Wt, Ht, wt_shift, tiles_x, tiles_y, BN; bool cols, pingpong; };
+static TilePlan plan_tiles(const femasr_tc_args* a, int H, int W, bool sliced = false) {
   static const int cols_env = [] { const char* e = getenv("FEMASR_TC_COLUMNS"); return e ? atoi(e) : 1; }();
+  static const int pp_env = [] { const char* e = getenv("FEMASR_TC_PINGPONG"); return e ? atoi(e) : 1; }();
   TilePlan t;
   t.BN = a->Cout % 128 == 0 ? 128 : 64;
   tc_tile_shape(H, W, &t.Wt, &t.Ht);   // the widest power-of-two Wt <= 128 that wastes the fewest padded pixels
@@ -1015,6 +1247,7 @@ static TilePlan plan_tiles(const femasr_tc_args* a, int H, int W) {
            (a->kb_count == 0 || a->kb_count == nkb) && cdiv(W, COL_WT) * cdiv(H, COL_HT) == (long)t.tiles_x * t.tiles_y;
   if (t.cols) { t.Wt = COL_WT; t.Ht = COL_HT; t.tiles_x = (int)cdiv(W, COL_WT); t.tiles_y = (int)cdiv(H, COL_HT); }
   t.wt_shift = 0; while ((1 << t.wt_shift) < t.Wt) ++t.wt_shift;
+  t.pingpong = pp_env && !sliced && t.BN == 64;
   return t;
 }
 
@@ -1253,7 +1486,12 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
   FEMASR_CHECK_ARG(!a->f8 || a->slice_kb == 0, "tc_igemm: the F8 cross-term mode is for the layers behind the VQ (no K slicing)");
   FEMASR_CHECK_ARG(!a->f8 || (a->ksize != 4 && a->ksize != 5 && a->act != FEMASR_ACT_LRELU),
                    "tc_igemm: no F8 cross-term mode for 4x4 / 5x5 convs or LeakyReLU");
-  const TilePlan plan = plan_tiles(a, H, W);
+  const int nkb_total = taps * (a->Cin / 64);
+  p.kb_begin = a->kb_begin; p.kb_end = a->kb_count > 0 ? a->kb_begin + a->kb_count : nkb_total;
+  FEMASR_CHECK_ARG(p.kb_begin >= 0 && p.kb_begin < p.kb_end && p.kb_end <= nkb_total, "tc_igemm: bad k-block slice");
+  FEMASR_CHECK_ARG(a->slice_kb >= 0, "tc_igemm: slice_kb must be >= 0");
+  p.slice_kb = (a->slice_kb > 0 && a->slice_kb < p.kb_end - p.kb_begin) ? a->slice_kb : 0;
+  const TilePlan plan = plan_tiles(a, H, W, p.slice_kb > 0);
   p.Wt = plan.Wt; p.Ht = plan.Ht; p.wt_shift = plan.wt_shift; p.tiles_x = plan.tiles_x; p.tiles_y = plan.tiles_y;
   const int BN = plan.BN;
   p.n_tiles = a->Cout / BN;
@@ -1261,11 +1499,6 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
   const long ntile = (long)phases * B * p.tiles_x * p.tiles_y * p.n_tiles;
   FEMASR_CHECK_ARG(ntile < (1l << 31), "tc_igemm: too many tiles");
   p.num_tiles = (int)ntile; p.cchunks = a->Cin / 64;
-  const int nkb_total = taps * p.cchunks;
-  p.kb_begin = a->kb_begin; p.kb_end = a->kb_count > 0 ? a->kb_begin + a->kb_count : nkb_total;
-  FEMASR_CHECK_ARG(p.kb_begin >= 0 && p.kb_begin < p.kb_end && p.kb_end <= nkb_total, "tc_igemm: bad k-block slice");
-  FEMASR_CHECK_ARG(a->slice_kb >= 0, "tc_igemm: slice_kb must be >= 0");
-  p.slice_kb = (a->slice_kb > 0 && a->slice_kb < p.kb_end - p.kb_begin) ? a->slice_kb : 0;
 
   CUtensorMap mah, mal, mbh, mbl;
   {
@@ -1290,5 +1523,5 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
   }
   cudaStream_t st = as_stream(stream);
   if (BN == 128) return launch_tc<128>(mah, mal, mbh, mbl, p, plan.cols, st);
-  return launch_tc<64>(mah, mal, mbh, mbl, p, plan.cols, st);
+  return plan.pingpong ? launch_tc<64, true>(mah, mal, mbh, mbl, p, plan.cols, st) : launch_tc<64, false>(mah, mal, mbh, mbl, p, plan.cols, st);
 }

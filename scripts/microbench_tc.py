@@ -11,6 +11,16 @@ if os.environ.get('MB_COLUMNS') == 'ab':
         env = dict(os.environ, MB_COLUMNS='', MB_F8='1', MB_ONLY=os.environ.get('MB_ONLY') or 'conv', FEMASR_TC_COLUMNS=v)
         subprocess.run([sys.executable, os.path.abspath(__file__)], env=env, check=True)
     sys.exit(0)
+# MB_PINGPONG=ab: the cases the ping-pong schedule runs (BN 64; BN 128 with no F8 / K-slice accumulator) on it
+# (FEMASR_TC_PINGPONG=1) and on the cooperative one (=0), the 3x3 convs in F8 mode with GroupNorm partials as in the
+# network; the K-sliced fc2 runs the cooperative schedule both times (a control)
+if os.environ.get('MB_PINGPONG') == 'ab':
+    for v in ('1', '0'):
+        print(f"# FEMASR_TC_PINGPONG={v}", flush=True)
+        env = dict(os.environ, MB_PINGPONG='', MB_F8='1', MB_GN='1', FEMASR_TC_PINGPONG=v,
+                   MB_ONLY=os.environ.get('MB_ONLY') or 'qkv|proj|fc1|fc2|64->64 @512|up 128->64')
+        subprocess.run([sys.executable, os.path.abspath(__file__)], env=env, check=True)
+    sys.exit(0)
 
 import torch
 
@@ -36,13 +46,13 @@ def timeit(fn, reps=5):
 
 PAIR = int(os.environ.get('MB_PAIR', '-1'))
 STRIP = int(os.environ.get('MB_STRIP', '-1'))
-ONLY = os.environ.get('MB_ONLY', '')        # substring filter on the case name
+ONLY = os.environ.get('MB_ONLY', '')        # substring filter on the case name ('|' separates alternatives)
 F8 = int(os.environ.get('MB_F8', '0'))      # 1: the 3x3 convs in the F8 cross-term mode (layers behind the VQ)
 GN = int(os.environ.get('MB_GN', '0'))      # 1: the 3x3 convs also emit GroupNorm partial sums (what most of them do in the network)
 
 
 def conv_case(name, B, H, W, Cin, Cout, ksize=3, up=0, res=False, act=0, split=False, bias=True, slice_kb=0):
-    if ONLY and ONLY not in name:
+    if ONLY and not any(o in name for o in ONLY.split('|')):
         return 0.0
     hi = (torch.randn(B, H, W, Cin, device=dev) * 0.5).half()
     lo = (torch.randn(B, H, W, Cin, device=dev) * 1e-4).half()
@@ -91,7 +101,7 @@ conv_case("up 128->64 @256->512", 32, 256, 256, 128, 64, up=1)
 
 
 def prep_case(name, B, H, W, C, mode):
-    if ONLY and ONLY not in name:
+    if ONLY and not any(o in name for o in ONLY.split('|')):
         return
     from femasr_b200 import lib as L
     x = torch.randn(B, H, W, C, device=dev)
