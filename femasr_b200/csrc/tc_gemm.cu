@@ -100,8 +100,7 @@ __device__ __forceinline__ bool elect_one() {
 // wgmma: D (registers of the warpgroup) += A (shared, K-major) x B (shared, K-major).  `accumulate` = 0 overwrites D.
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // Named barriers of the ping-pong schedule, and the per-warpgroup register budgets (setmaxnreg, one whole warpgroup)
 __device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
@@ -194,7 +193,7 @@ constexpr int TC_CONSUMER_WARPS = 8, TC_THREADS = 32 * TC_CONSUMER_WARPS + 32;
 // registers to the consumers: 128 x 40 + 256 x 232 = 64512 <= 65536, the 168 per thread of the launch.
 constexpr int TC_PP_THREADS = 32 * TC_CONSUMER_WARPS + 128;
 constexpr int PP_PRODUCER_REGS = 40, PP_CONSUMER_REGS = 232;
-constexpr int PP_GN_BAR = 2, PP_ORDER_BAR = 4;     // named barriers (+ warpgroup); 1 is the cooperative epilogue's
+constexpr int TC_GN_BAR = 1, PP_GN_BAR = 2, PP_ORDER_BAR = 4;   // named barriers (PP: + warpgroup)
 constexpr int TC_SMEM_LIMIT = 232448;              // 227 KB of opt-in shared memory per block on H100
 
 // Column schedule (COLS): 8 x 16 output tiles; one activation box of 64 ch x 8 cols x 18 rows per (channel chunk, dx)
@@ -235,35 +234,230 @@ __device__ __forceinline__ void top4_insert(float (&td)[4], int (&tj)[4], float 
     }
 }
 
+// it-th work item of this CTA (-1: done).  Default: items strided over the CTAs.  VQ: m-tiles strided over the CTAs, and
+// for each m-tile every n-tile (code tile) in turn.
+template <bool VQ>
+__device__ __forceinline__ int work_of(const TcP& p, int it) {
+  if (VQ) {
+    const int mt = (it / p.n_tiles) * (int)gridDim.x + (int)blockIdx.x;
+    return mt < p.num_tiles / p.n_tiles ? mt * p.n_tiles + it % p.n_tiles : -1;
+  }
+  const int w = (int)blockIdx.x + it * (int)gridDim.x;
+  return w < p.num_tiles ? w : -1;
+}
+// work item -> (n-tile, m-tile); the m-tile decodes into (phase, image, tile row/col)
+struct TileCoord { int nt, tx, ty, b, ph; };
+__device__ __forceinline__ TileCoord decode_tile(const TcP& p, int work) {
+  TileCoord tc;
+  tc.nt = work % p.n_tiles;
+  int mt = work / p.n_tiles;
+  tc.tx = mt % p.tiles_x; mt /= p.tiles_x;
+  tc.ty = mt % p.tiles_y; mt /= p.tiles_y;
+  tc.b = mt % p.B;
+  tc.ph = mt / p.B;                                // sub-pixel phase (0 unless p.up)
+  return tc;
+}
+
+// The CTA's rings (TcCfg): operand addresses and mbarriers (full / empty per stage, then per column box)
+template <class Cfg>
+struct Rings {
+  uint32_t smem_base, bar_base;
+  __device__ __forceinline__ uint32_t stage(int s) const { return smem_base + Cfg::COL_RING_BYTES + s * Cfg::STAGE_BYTES; }
+  __device__ __forceinline__ uint32_t column(int s) const { return smem_base + s * COL_STAGE_BYTES; }
+  __device__ __forceinline__ uint32_t full(int s) const { return bar_base + 8u * s; }
+  __device__ __forceinline__ uint32_t empty(int s) const { return bar_base + 8u * (Cfg::STAGES + s); }
+  __device__ __forceinline__ uint32_t col_full(int s) const { return bar_base + 8u * (2 * Cfg::STAGES + s); }
+  __device__ __forceinline__ uint32_t col_empty(int s) const { return bar_base + 8u * (2 * Cfg::STAGES + Cfg::COL_STAGES + s); }
+};
+
+// ---------------------------------------------------------------- TMA producer (one elected lane)
+// Column schedule: per (chunk, dx) the column box at (x + dx, y - 1), then the weight boxes of taps (-1, dx), (0, dx), (+1, dx)
+template <int BN, class Cfg>
+__device__ __forceinline__ void produce_columns(const TcP& p, const Rings<Cfg>& r, const CUtensorMap* map_a_hi,
+                                                const CUtensorMap* map_a_lo, const CUtensorMap* map_b_hi,
+                                                const CUtensorMap* map_b_lo) {
+  int stage = 0, cstage = 0; uint32_t phase = 0, cphase = 0;
+  for (int it = 0, work; (work = work_of<false>(p, it)) >= 0; ++it) {
+    const TileCoord tc = decode_tile(p, work);
+    const int n0 = tc.nt * BN, x0 = tc.tx * COL_WT, y0 = tc.ty * COL_HT - 1;
+    for (int c0 = 0; c0 < p.Cin; c0 += TC_BK) {
+      for (int dx = 0; dx < 3; ++dx) {
+        mbar_wait(r.col_empty(cstage), cphase ^ 1u);
+        const uint32_t ca = r.column(cstage);
+        mbar_expect_tx(r.col_full(cstage), COL_STAGE_BYTES);
+        tma_load_4d(ca, map_a_hi, r.col_full(cstage), c0, x0 + dx - 1, y0, tc.b);
+        tma_load_4d(ca + COL_PLANE_BYTES, map_a_lo, r.col_full(cstage), c0, x0 + dx - 1, y0, tc.b);
+        if (++cstage == Cfg::COL_STAGES) { cstage = 0; cphase ^= 1u; }
+        for (int dy = 0; dy < 3; ++dy) {
+          const int k0 = (3 * dy + dx) * p.Cin + c0;
+          mbar_wait(r.empty(stage), phase ^ 1u);
+          const uint32_t sb = r.stage(stage);
+          mbar_expect_tx(r.full(stage), Cfg::STAGE_BYTES);
+          tma_load_2d(sb, map_b_hi, r.full(stage), k0, n0);
+          tma_load_2d(sb + Cfg::B_PLANE_BYTES, map_b_lo, r.full(stage), k0, n0);
+          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1u; }
+        }
+      }
+    }
+  }
+}
+
+// Tap order: per k-block the activation box of its channel chunk at its tap's spatial offset (conv padding = TMA zero
+// fill) and its weight boxes
+template <int BN, bool VQ, int EXT, class Cfg>
+__device__ __forceinline__ void produce_taps(const TcP& p, const Rings<Cfg>& r, const CUtensorMap* map_a_hi,
+                                             const CUtensorMap* map_a_lo, const CUtensorMap* map_b_hi,
+                                             const CUtensorMap* map_b_lo) {
+  const int ksz = EXT == 1 && p.taps == 16 ? 4 : EXT == 2 && p.taps == 25 ? 5 : (p.taps == 9 ? 3 : 1);   // (p.up: taps == 4)
+  int stage = 0; uint32_t phase = 0;
+  for (int it = 0, work; (work = work_of<VQ>(p, it)) >= 0; ++it) {
+    const TileCoord tc = decode_tile(p, work);
+    const int n0 = tc.ph * p.Cout + tc.nt * BN;
+    for (int kb = p.kb_begin; kb < p.kb_end; ++kb) {
+      const int tap = kb / p.cchunks;
+      const int c0 = (kb - tap * p.cchunks) * TC_BK;
+      int dy = 0, dx = 0;
+      if (p.up) { dy = (tap >> 1) - 1 + (tc.ph >> 1); dx = (tap & 1) - 1 + (tc.ph & 1); }
+      else if (ksz == 3) { dy = tap / 3 - 1; dx = tap - (tap / 3) * 3 - 1; }
+      else if (EXT == 1 && ksz == 4) { dy = (tap >> 2) - 1; dx = (tap & 3) - 1; }     // 4x4 pad 1, always stride 2
+      else if (EXT == 2 && ksz == 5) { dy = tap / 5 - 2; dx = tap % 5 - 2; }          // 5x5 pad 2, stride 1
+      const int x = p.stride * tc.tx * p.Wt + dx, y = p.stride * tc.ty * p.Ht + dy;
+      mbar_wait(r.empty(stage), phase ^ 1u);
+      const uint32_t sa = r.stage(stage);
+      mbar_expect_tx(r.full(stage), Cfg::STAGE_BYTES);
+      tma_load_4d(sa, map_a_hi, r.full(stage), c0, x, y, tc.b);
+      tma_load_4d(sa + A_PLANE_BYTES, map_a_lo, r.full(stage), c0, x, y, tc.b);
+      tma_load_2d(sa + 2 * A_PLANE_BYTES, map_b_hi, r.full(stage), tap * p.Cin + c0, n0);
+      tma_load_2d(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES, map_b_lo, r.full(stage), tap * p.Cin + c0, n0);
+      if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1u; }
+    }
+  }
+}
+
+// ---------------------------------------------------------------- consumers
+// A consumer warpgroup's accumulators are NH m64 halves (cooperative 1, PP 2) of BN / 2 floats per thread; ext holds the
+// F8 cross products (cooperative: or the running sum of the K slices).
+template <bool F8, int NH, int NF>
+__device__ __forceinline__ void fence_acc(float (&acc)[NH][NF], float (&ext)[NH][NF]) {
+#pragma unroll
+  for (int h = 0; h < NH; ++h) fence_regs(acc[h]);
+  if (F8) {
+#pragma unroll
+    for (int h = 0; h < NH; ++h) fence_regs(ext[h]);
+  }
+}
+
+// One k-block (K = 64) of wgmmas into the NH halves (A rows A_PLANE_BYTES / 2 apart), small cross terms first and the
+// dominant hi * hi product last: F8, the e4m3 cross term (sum a_lo8 w_hi8 + sum a_hi8 w_lo8) into ext, then hi * hi;
+// fp16, lo * hi, hi * lo, hi * hi.  more = 0 starts the accumulators afresh.  Returns once at most WAIT committed
+// k-blocks of wgmmas are still running.
+template <int BN, bool F8, int NH, int WAIT>
+__device__ __forceinline__ void mma_kblock(float (&acc)[NH][BN / 2], float (&ext)[NH][BN / 2], uint32_t a_hi_addr,
+                                           uint32_t a_lo_addr, uint32_t b_addr, uint32_t more) {
+  const uint64_t b_hi = make_sw128_desc(b_addr);
+  const uint64_t b_lo = make_sw128_desc(b_addr + TcCfg<BN>::B_PLANE_BYTES);
+  fence_acc<F8>(acc, ext);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < TC_BK / 16; ++k) {
+    const uint64_t ko = (uint64_t)((k * 32) >> 4);   // +32 bytes per k-step inside the 128B swizzle atom
+    const uint32_t m = k ? 1u : more;
+#pragma unroll
+    for (int h = 0; h < NH; ++h) {
+      const uint64_t a_hi = make_sw128_desc(a_hi_addr + h * (A_PLANE_BYTES / 2));
+      const uint64_t a_lo = make_sw128_desc(a_lo_addr + h * (A_PLANE_BYTES / 2));
+      if constexpr (F8) {
+        Wgmma<BN>::e4m3(ext[h], a_lo + ko, b_lo + ko, m);
+        Wgmma<BN>::f16(acc[h], a_hi + ko, b_hi + ko, m);
+      } else {
+        Wgmma<BN>::f16(acc[h], a_lo + ko, b_hi + ko, m);
+        Wgmma<BN>::f16(acc[h], a_hi + ko, b_lo + ko, 1u);
+        Wgmma<BN>::f16(acc[h], a_hi + ko, b_hi + ko, 1u);
+      }
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<WAIT>();
+  fence_acc<F8>(acc, ext);
+}
+
+// A consumer's position in the rings: the next stage and its parity, and the column boxes consumed
+struct RingPos {
+  int stage = 0; uint32_t phase = 0, ncol = 0;
+  template <int STAGES> __device__ __forceinline__ void next() { if (++stage == STAGES) { stage = 0; phase ^= 1u; } }
+};
+
+// The k-blocks of one work item, in the column schedule's order channel chunk, dx, dy: kblock(a_hi, a_lo, b, more,
+// stage, col) once each stage is full; the A operand of tap dy starts 8 (dy + 1) rows into the column box, and col is
+// the box's slot at its third tap (the box is free once that k-block has read it), else -1.
+template <class Cfg, class KBlock>
+__device__ __forceinline__ void walk_columns(const TcP& p, const Rings<Cfg>& r, RingPos& pos, KBlock&& kblock) {
+  for (int col = 0; col < 3 * p.cchunks; ++col, ++pos.ncol) {        // (chunk, dx) in that order
+    const int cs = pos.ncol % Cfg::COL_STAGES;
+    mbar_wait(r.col_full(cs), (pos.ncol / Cfg::COL_STAGES) & 1u);
+    const uint32_t ca = r.column(cs);
+#pragma unroll 1
+    for (int dy = 0; dy < 3; ++dy) {
+      mbar_wait(r.full(pos.stage), pos.phase);
+      kblock(ca + 1024 * dy, ca + COL_PLANE_BYTES + 1024 * dy, r.stage(pos.stage), col || dy ? 1u : 0u, pos.stage,
+             dy == 2 ? cs : -1);
+      pos.next<Cfg::STAGES>();
+    }
+  }
+}
+
+// The k-blocks kb_begin .. kb_end - 1 of one work item in tap order: kblock(a_hi, a_lo, b, more, stage, -1) once each
+// stage is full.  SLICED (cooperative): in slices of slice_len, more = 0 at the first k-block of each and fold() after
+// every slice but the last; otherwise (PP, never K-sliced) one slice, a loop ptxas compiles without the slice bookkeeping.
+template <bool SLICED, class Cfg, class KBlock, class Fold>
+__device__ __forceinline__ void walk_taps(const TcP& p, const Rings<Cfg>& r, RingPos& pos, int slice_len, KBlock&& kblock,
+                                          Fold&& fold) {
+  for (int kb0 = p.kb_begin; kb0 < p.kb_end; kb0 = SLICED ? kb0 + slice_len : p.kb_end) {
+    const int kb1 = SLICED ? min(kb0 + slice_len, p.kb_end) : p.kb_end;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(r.full(pos.stage), pos.phase);
+      const uint32_t sa = r.stage(pos.stage);
+      kblock(sa, sa + A_PLANE_BYTES, sa + 2 * A_PLANE_BYTES, kb != kb0 ? 1u : 0u, pos.stage, -1);
+      pos.next<Cfg::STAGES>();
+    }
+    if (SLICED && kb1 < p.kb_end) fold();
+  }
+}
+
 // Epilogue of one warp's 16 accumulator rows of a tile (rows row0 + lane / 4 and row0 + lane / 4 + 8):
 // acc * 2^-s + bias -> GELU | ReLU -> + res1 + res2 -> store.  With GroupNorm partials, the warp's per-group sum and sum
-// of squares over its 16 rows go to red_row[2 g], red_row[2 g + 1].  Used by the ping-pong schedule (BN 64).  The
-// cooperative schedule keeps its inline copy, which loads each residual inside the store loop: calling this helper there
-// changes ptxas's allocation in every cooperative instantiation, and at BN 128 the residual registers spill.  Both copies
-// compute the same values (tests/test_tc_pingpong_gpu.py compares bytes).
-template <int BN, bool RES, int EXT, class TileCoord>
+// of squares over its 16 rows go to red[2 (red_slot + g)], red[2 (red_slot + g) + 1] (a slot index rather than a row
+// pointer: the pointer would stay live through the store loop, +2 registers in the cooperative BN-64 instantiations).
+// PREFETCH_RES: the thread's residuals are all loaded before its first store.  As far as the compiler knows the stores
+// may alias res1 (they do in the in-place residual convs), so a load issued inside the store loop waits for the previous
+// stores and pays one memory round trip per column block and row; each element is still read before its own store.  The
+// ping-pong schedule prefetches.  The cooperative one loads inside the store loop: at BN 128 its 168 registers hold the
+// F8 / K-slice accumulator beside the tile's, and the prefetched residual spills.  Both compute the same values.
+template <int BN, bool RES, int EXT, bool PREFETCH_RES>
 __device__ __forceinline__ void epilogue_rows(const TcP& p, const TileCoord& tc, const float (&acc)[BN / 2], int row0,
-                                              float inv_scale, float* red_row, int lane) {
+                                              float inv_scale, float* red, int red_slot, int lane) {
   const int rsub = lane >> 2, q = lane & 3;
   const int Ho = p.up ? 2 * p.H : p.H, Wo = p.up ? 2 * p.W : p.W;
-  long off[2];                                         // output element offset of this thread's two rows (-1: outside)
+  // off: the output element offset of this thread's two rows (-1: outside).  At BN 128 it includes the thread's first
+  // column (tc.nt * BN + 2 q), so that column block j adds the constant 8 j instead of sign-extending its column to 64
+  // bits per element (~230 fewer instructions in the cooperative residual kernels).  At BN 64 the column stays out: folded
+  // in, it costs the cooperative kernels 2 registers.
+  constexpr bool FOLD_COL = BN == 128;
+  long off[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int row = row0 + rsub + 8 * h;
     const int y = tc.ty * p.Ht + (row >> p.wt_shift), x = tc.tx * p.Wt + (row & (p.Wt - 1));
     const int oy = p.up ? 2 * y + (tc.ph >> 1) : y, ox = p.up ? 2 * x + (tc.ph & 1) : x;
-    off[h] = (y < p.H && x < p.W) ? (((long)tc.b * Ho + oy) * Wo + ox) * p.Cout : -1;
+    off[h] = (y < p.H && x < p.W) ? (((long)tc.b * Ho + oy) * Wo + ox) * p.Cout + (FOLD_COL ? tc.nt * BN + 2 * q : 0) : -1;
   }
-  // The thread's residuals are all loaded before its first store.  As far as the compiler knows the stores may alias
-  // res1 (they do in the in-place residual convs), so a load issued inside the store loop would wait for the previous
-  // stores and pay one memory round trip per column block and row.  Each element is still read before its own store.
-  float2 r1[RES ? BN / 8 : 1][2];
-  if constexpr (RES) {
+  float2 r1[RES && PREFETCH_RES ? BN / 8 : 1][2];
+  if constexpr (RES && PREFETCH_RES) {
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
       for (int h = 0; h < 2; ++h)
-        r1[j][h] = off[h] >= 0 ? *reinterpret_cast<const float2*>(p.res1 + off[h] + tc.nt * BN + 8 * j + 2 * q)
+        r1[j][h] = off[h] >= 0 ? *reinterpret_cast<const float2*>(p.res1 + off[h] + (FOLD_COL ? 8 * j : tc.nt * BN + 8 * j + 2 * q))
                                : make_float2(0.f, 0.f);
   }
 #pragma unroll
@@ -280,8 +474,11 @@ __device__ __forceinline__ void epilogue_rows(const TcP& p, const TileCoord& tc,
       else if (p.act == FEMASR_ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
       else if (EXT == 1 && p.act == FEMASR_ACT_LRELU) { o.x = lrelu02_f(o.x); o.y = lrelu02_f(o.y); }
       if (off[h] >= 0) {
-        const long o_off = off[h] + col;
-        if (RES) { o.x += r1[j][h].x; o.y += r1[j][h].y; }
+        const long o_off = off[h] + (FOLD_COL ? 8 * j : col);
+        if (RES) {
+          const float2 r = PREFETCH_RES ? r1[j][h] : *reinterpret_cast<const float2*>(p.res1 + o_off);
+          o.x += r.x; o.y += r.y;
+        }
         if (p.res2) { const float2 r = *reinterpret_cast<const float2*>(p.res2 + o_off); o.x += r.x; o.y += r.y; }
         if (p.out_hi) {
           uint32_t hh, ll;
@@ -302,18 +499,20 @@ __device__ __forceinline__ void epilogue_rows(const TcP& p, const TileCoord& tc,
       if (p.cpg >= 8) { gs += __shfl_xor_sync(0xffffffffu, gs, 2); gss += __shfl_xor_sync(0xffffffffu, gss, 2); }
       if (rsub == 0 && (q & (p.cpg / 2 - 1)) == 0) {
         const int g = (8 * j + 2 * q) / p.cpg;
-        red_row[g * 2] = gs;
-        red_row[g * 2 + 1] = gss;
+        red[(red_slot + g) * 2] = gs;
+        red[(red_slot + g) * 2 + 1] = gss;
       }
     }
   }
 }
 
 // One GroupNorm partial row per 32-row quarter of the tile: the sum of the two 16-row warp partials that cover it, in
-// that order.  red holds the warp partials of 16-row group k at red[2 (k * gslots + g)]; threads tid = 0 .. nthreads - 1.
-template <int BN, class TileCoord>
+// that order.  red holds the warp partials of 16-row group k at red[2 (k * gslots + g)]; the nthreads threads
+// tid = 0 .. nthreads - 1 that wrote them meet at named barrier bar before and after.
+template <int BN>
 __device__ __forceinline__ void gn_store_partials(const TcP& p, const TileCoord& tc, const float* red, int gslots, int tid,
-                                                  int nthreads) {
+                                                  int nthreads, int bar) {
+  named_bar_sync(bar, nthreads);
   const int gpl = BN / p.cpg;                           // GroupNorm groups of this n-tile
   const int tile_in_img = (tc.ph * p.tiles_y + tc.ty) * p.tiles_x + tc.tx;
   for (int i = tid; i < 4 * gpl; i += nthreads) {
@@ -323,6 +522,7 @@ __device__ __forceinline__ void gn_store_partials(const TcP& p, const TileCoord&
     float* gp = p.gn_partial + (((long)tc.b * p.gn_rows + tile_in_img * 4 + quarter) * 32 + tc.nt * gpl + g) * 2;
     *reinterpret_cast<float2*>(gp) = make_float2(r0[0] + r1[0], r0[1] + r1[1]);
   }
+  named_bar_sync(bar, nthreads);
 }
 
 // RES: the layer adds a residual tile (res1) in the epilogue (a template parameter: the load is in the hot loop).
@@ -337,125 +537,50 @@ __device__ __forceinline__ void gn_store_partials(const TcP& p, const TileCoord&
 // order channel chunk, dx, dy, over the whole K range.
 // PP: the ping-pong schedule (TC_PP_THREADS) of the BN-64 launches: each consumer warpgroup owns whole 128-row tiles,
 // the two take turns on the tensor cores, and one runs its epilogue while the other runs its k-loop (plan_tiles).
+// Both schedules issue their k-blocks through mma_kblock, walk the rings with walk_columns / walk_taps and store through
+// epilogue_rows and gn_store_partials; they differ in how many k-blocks stay in flight and where a stage is released.
 template <int BN, bool RES, bool F8, bool VQ = false, int EXT = 0, bool COLS = false, bool PP = false>
 __global__ void __launch_bounds__(PP ? TC_PP_THREADS : TC_THREADS, 1)
 tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                 const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const TcP p) {
   using Cfg = TcCfg<BN, COLS>;
-  constexpr int STAGES = Cfg::STAGES, COL_STAGES = Cfg::COL_STAGES, NF = Cfg::NF;
+  constexpr int NF = Cfg::NF;
   static_assert(!VQ || (!RES && !F8), "VQ mode: plain linear tiles");
   static_assert(!COLS || (F8 && !VQ && EXT == 0), "column schedule: F8 3x3 convs");
   static_assert(!PP || (BN == 64 && !VQ), "ping-pong schedule: BN-64 convs and linears");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t ring_base = smem_base + Cfg::COL_RING_BYTES;      // the stage ring
-  const uint32_t bar_base = smem_base + Cfg::RING_BYTES;
-  float* red = reinterpret_cast<float*>(smem_raw + (bar_base + 256u - smem_u32(smem_raw)));
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto col_full_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-  auto col_empty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + COL_STAGES + s); };
-
-  const int worker = (int)blockIdx.x, nworkers = (int)gridDim.x;
-  const int num_m = p.num_tiles / p.n_tiles;
-  // it-th work item of this CTA (-1: done).  Default: items strided over the CTAs.  VQ: m-tiles strided over the
-  // CTAs, and for each m-tile every n-tile (code tile) in turn.
-  auto work_of = [&](int it) -> int {
-    if (VQ) {
-      const int mt = (it / p.n_tiles) * nworkers + worker;
-      return mt < num_m ? mt * p.n_tiles + it % p.n_tiles : -1;
-    }
-    const int w = worker + it * nworkers;
-    return w < p.num_tiles ? w : -1;
-  };
-  // work item -> (n-tile, m-tile); the m-tile decodes into (phase, image, tile row/col)
-  struct TileCoord { int nt, tx, ty, b, ph; };
-  auto decode = [&](int work) {
-    TileCoord tc;
-    tc.nt = work % p.n_tiles;
-    int mt = work / p.n_tiles;
-    tc.tx = mt % p.tiles_x; mt /= p.tiles_x;
-    tc.ty = mt % p.tiles_y; mt /= p.tiles_y;
-    tc.b = mt % p.B;
-    tc.ph = mt / p.B;                                // sub-pixel phase (0 unless p.up)
-    return tc;
-  };
+  const Rings<Cfg> r{smem_base, smem_base + Cfg::RING_BYTES};
+  float* red = reinterpret_cast<float*>(smem_raw + (r.bar_base + 256u - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   pdl_launch_dependents();        // the next kernel of the stream may begin its own prologue as our CTAs retire
   if (threadIdx.x == 0) {
     // a stage (column box) is released by every warp that reads it: all consumer warps, or (PP) one warpgroup's
     constexpr int READERS = PP ? TC_CONSUMER_WARPS / 2 : TC_CONSUMER_WARPS;
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), READERS); }
-    for (int s = 0; s < COL_STAGES; ++s) { mbar_init(col_full_bar(s), 1); mbar_init(col_empty_bar(s), READERS); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(r.full(s), 1); mbar_init(r.empty(s), READERS); }
+    for (int s = 0; s < Cfg::COL_STAGES; ++s) { mbar_init(r.col_full(s), 1); mbar_init(r.col_empty(s), READERS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   pdl_wait();                     // barriers initialised: from here on the predecessor's output is read
 
   if (PP ? warp >= TC_CONSUMER_WARPS : warp == TC_CONSUMER_WARPS) {
-    // ===================== TMA producer =====================
     if constexpr (PP) {
       setmaxnreg_dec<PP_PRODUCER_REGS>();      // the whole warpgroup; one lane of its first warp issues the loads
       if (warp != TC_CONSUMER_WARPS) return;
     }
     if (!elect_one()) return;
-    if constexpr (COLS) {
-      // per (chunk, dx): the column box at (x + dx, y - 1), then the weight boxes of taps (-1, dx), (0, dx), (+1, dx)
-      int stage = 0, cstage = 0; uint32_t phase = 0, cphase = 0;
-      for (int it = 0, work; (work = work_of(it)) >= 0; ++it) {
-        const TileCoord tc = decode(work);
-        const int n0 = tc.nt * BN, x0 = tc.tx * COL_WT, y0 = tc.ty * COL_HT - 1;
-        for (int c0 = 0; c0 < p.Cin; c0 += TC_BK) {
-          for (int dx = 0; dx < 3; ++dx) {
-            mbar_wait(col_empty_bar(cstage), cphase ^ 1u);
-            const uint32_t ca = smem_base + cstage * COL_STAGE_BYTES;
-            mbar_expect_tx(col_full_bar(cstage), COL_STAGE_BYTES);
-            tma_load_4d(ca, &map_a_hi, col_full_bar(cstage), c0, x0 + dx - 1, y0, tc.b);
-            tma_load_4d(ca + COL_PLANE_BYTES, &map_a_lo, col_full_bar(cstage), c0, x0 + dx - 1, y0, tc.b);
-            if (++cstage == COL_STAGES) { cstage = 0; cphase ^= 1u; }
-            for (int dy = 0; dy < 3; ++dy) {
-              const int k0 = (3 * dy + dx) * p.Cin + c0;
-              mbar_wait(empty_bar(stage), phase ^ 1u);
-              const uint32_t sb = ring_base + stage * Cfg::STAGE_BYTES;
-              mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-              tma_load_2d(sb, &map_b_hi, full_bar(stage), k0, n0);
-              tma_load_2d(sb + Cfg::B_PLANE_BYTES, &map_b_lo, full_bar(stage), k0, n0);
-              if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-            }
-          }
-        }
-      }
-      return;
-    }
-    const int ksz = EXT == 1 && p.taps == 16 ? 4 : EXT == 2 && p.taps == 25 ? 5 : (p.taps == 9 ? 3 : 1);   // (p.up: taps == 4)
-    int stage = 0; uint32_t phase = 0;
-    for (int it = 0, work; (work = work_of(it)) >= 0; ++it) {
-      const TileCoord tc = decode(work);
-      const int n0 = tc.ph * p.Cout + tc.nt * BN;
-      for (int kb = p.kb_begin; kb < p.kb_end; ++kb) {
-        // activation box of k-block kb: channel chunk and the tap's spatial offset (conv padding = TMA zero fill)
-        const int tap = kb / p.cchunks;
-        const int c0 = (kb - tap * p.cchunks) * TC_BK;
-        int dy = 0, dx = 0;
-        if (p.up) { dy = (tap >> 1) - 1 + (tc.ph >> 1); dx = (tap & 1) - 1 + (tc.ph & 1); }
-        else if (ksz == 3) { dy = tap / 3 - 1; dx = tap - (tap / 3) * 3 - 1; }
-        else if (EXT == 1 && ksz == 4) { dy = (tap >> 2) - 1; dx = (tap & 3) - 1; }     // 4x4 pad 1, always stride 2
-        else if (EXT == 2 && ksz == 5) { dy = tap / 5 - 2; dx = tap % 5 - 2; }          // 5x5 pad 2, stride 1
-        const int x = p.stride * tc.tx * p.Wt + dx, y = p.stride * tc.ty * p.Ht + dy;
-        mbar_wait(empty_bar(stage), phase ^ 1u);
-        const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-        mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-        tma_load_4d(sa, &map_a_hi, full_bar(stage), c0, x, y, tc.b);
-        tma_load_4d(sa + A_PLANE_BYTES, &map_a_lo, full_bar(stage), c0, x, y, tc.b);
-        tma_load_2d(sa + 2 * A_PLANE_BYTES, &map_b_hi, full_bar(stage), tap * p.Cin + c0, n0);
-        tma_load_2d(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES, &map_b_lo, full_bar(stage), tap * p.Cin + c0, n0);
-        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-      }
-    }
+    if constexpr (COLS) produce_columns<BN>(p, r, &map_a_hi, &map_a_lo, &map_b_hi, &map_b_lo);
+    else produce_taps<BN, VQ, EXT>(p, r, &map_a_hi, &map_a_lo, &map_b_hi, &map_b_lo);
     return;
   }
 
+  // Accumulator fragment of m64nBNk16 (per warp 16 rows): d[4j + 2h + e] = row 16 * (warp % 4) + lane / 4 + 8h,
+  // column 8j + 2 (lane % 4) + e.
+  const int wg = warp >> 2;
+  const float inv_scale = __ldg(p.inv_scale);
+  RingPos pos;
   if constexpr (PP) {
     // ===================== ping-pong consumers: warpgroup wg takes work items it = wg, wg + 2, ... =====================
     // Both halves of the tile (rows 0-63, 64-127) are m64 accumulators of the same warpgroup, each summed in the same
@@ -464,20 +589,16 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
     // barrier (PP_ORDER_BAR + wg) hands the tensor cores over at the end of each k-loop: the other warpgroup's k-loop
     // then overlaps this one's epilogue.
     setmaxnreg_inc<PP_CONSUMER_REGS>();
-    const int wg = warp >> 2;
-    const float inv_scale = __ldg(p.inv_scale);
     const int nkb = COLS ? 9 * p.cchunks : p.kb_end - p.kb_begin;   // k-blocks per work item
-    int stage = 0; uint32_t phase = 0;
-    uint32_t ncol = 0;                     // COLS: column boxes consumed (the column ring's position)
     auto skip_item = [&]() {
-      stage += nkb;
-      while (stage >= STAGES) { stage -= STAGES; phase ^= 1u; }
-      if (COLS) ncol += 3 * p.cchunks;
+      pos.stage += nkb;
+      while (pos.stage >= Cfg::STAGES) { pos.stage -= Cfg::STAGES; pos.phase ^= 1u; }
+      if (COLS) pos.ncol += 3 * p.cchunks;
     };
     if (wg == 1) skip_item();
     float* red_wg = red + wg * 8 * 32 * 2;   // 8 groups of 16 rows x at most 32 GroupNorm groups per warpgroup
-    for (int it = wg, work; (work = work_of(it)) >= 0; it += 2) {
-      const TileCoord tc = decode(work);
+    for (int it = wg, work; (work = work_of<VQ>(p, it)) >= 0; it += 2) {
+      const TileCoord tc = decode_tile(p, work);
       float acc[2][NF], ext[2][NF];
       if (it > 0) named_bar_sync(PP_ORDER_BAR + wg, 256);     // the previous item's k-loop is issued
       // One k-block of wgmmas stays in flight: a stage (and a column box after its third tap) is released once the
@@ -486,66 +607,20 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
       auto release = [&]() {
         __syncwarp();
         if (lane == 0) {
-          if (rel_stage >= 0) mbar_arrive(empty_bar(rel_stage));
-          if (rel_col >= 0) mbar_arrive(col_empty_bar(rel_col));
+          if (rel_stage >= 0) mbar_arrive(r.empty(rel_stage));
+          if (rel_col >= 0) mbar_arrive(r.col_empty(rel_col));
         }
       };
-      auto kblock = [&](uint32_t a0, uint32_t a1, uint32_t b_addr, uint32_t more) {
-        const uint64_t b_hi = make_sw128_desc(b_addr);
-        const uint64_t b_lo = make_sw128_desc(b_addr + Cfg::B_PLANE_BYTES);
-        fence_regs(acc[0]); fence_regs(acc[1]);
-        if (F8) { fence_regs(ext[0]); fence_regs(ext[1]); }
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k) {
-          const uint64_t ko = (uint64_t)((k * 32) >> 4);
-          const uint32_t m = k ? 1u : more;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint64_t a_hi = make_sw128_desc(a0 + h * (A_PLANE_BYTES / 2));
-            const uint64_t a_lo = make_sw128_desc(a1 + h * (A_PLANE_BYTES / 2));
-            if constexpr (F8) {
-              Wgmma<BN>::e4m3(ext[h], a_lo + ko, b_lo + ko, m);
-              Wgmma<BN>::f16(acc[h], a_hi + ko, b_hi + ko, m);
-            } else {
-              Wgmma<BN>::f16(acc[h], a_lo + ko, b_hi + ko, m);
-              Wgmma<BN>::f16(acc[h], a_hi + ko, b_lo + ko, 1u);
-              Wgmma<BN>::f16(acc[h], a_hi + ko, b_hi + ko, 1u);
-            }
-          }
-        }
-        wgmma_commit();
-        wgmma_wait_1();
-        fence_regs(acc[0]); fence_regs(acc[1]);
-        if (F8) { fence_regs(ext[0]); fence_regs(ext[1]); }
+      auto kblock = [&](uint32_t a_hi, uint32_t a_lo, uint32_t b, uint32_t more, int stage, int col) {
+        mma_kblock<BN, F8, 2, 1>(acc, ext, a_hi, a_lo, b, more);
         release();
+        rel_stage = stage; rel_col = col;
       };
-      if constexpr (COLS) {
-        for (int col = 0; col < 3 * p.cchunks; ++col, ++ncol) {        // (chunk, dx) in that order
-          const int cs = ncol % COL_STAGES;
-          mbar_wait(col_full_bar(cs), (ncol / COL_STAGES) & 1u);
-          const uint32_t ca = smem_base + cs * COL_STAGE_BYTES;
-#pragma unroll 1
-          for (int dy = 0; dy < 3; ++dy) {
-            mbar_wait(full_bar(stage), phase);
-            kblock(ca + 1024 * dy, ca + COL_PLANE_BYTES + 1024 * dy, ring_base + stage * Cfg::STAGE_BYTES, col || dy ? 1u : 0u);
-            rel_stage = stage; rel_col = dy == 2 ? cs : -1;
-            if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-          }
-        }
-      } else {
-        for (int kb = p.kb_begin; kb < p.kb_end; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          kblock(sa, sa + A_PLANE_BYTES, sa + 2 * A_PLANE_BYTES, kb != p.kb_begin ? 1u : 0u);
-          rel_stage = stage;
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-      if (work_of(it + 1) >= 0) named_bar_arrive(PP_ORDER_BAR + (wg ^ 1), 256);
-      wgmma_wait_all();
-      fence_regs(acc[0]); fence_regs(acc[1]);
-      if (F8) { fence_regs(ext[0]); fence_regs(ext[1]); }
+      if constexpr (COLS) walk_columns(p, r, pos, kblock);
+      else walk_taps<false>(p, r, pos, 0, kblock, [] {});
+      if (work_of<VQ>(p, it + 1) >= 0) named_bar_arrive(PP_ORDER_BAR + (wg ^ 1), 256);
+      wgmma_wait<0>();
+      fence_acc<F8>(acc, ext);
       release();
       skip_item();                                       // the other warpgroup's next item
       if (F8) {
@@ -558,115 +633,47 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
       // the cooperative schedule
 #pragma unroll
       for (int h = 0; h < 2; ++h)
-        epilogue_rows<BN, RES, EXT>(p, tc, acc[h], h * 64 + (warp & 3) * 16, inv_scale, red_wg + (4 * h + (warp & 3)) * 32 * 2, lane);
-      if (p.gn_partial) {
-        named_bar_sync(PP_GN_BAR + wg, 128);
-        gn_store_partials<BN>(p, tc, red_wg, 32, threadIdx.x & 127, 128);
-        named_bar_sync(PP_GN_BAR + wg, 128);
-      }
+        epilogue_rows<BN, RES, EXT, true>(p, tc, acc[h], h * 64 + (warp & 3) * 16, inv_scale,
+                                          red_wg, (4 * h + (warp & 3)) * 32, lane);
+      if (p.gn_partial) gn_store_partials<BN>(p, tc, red_wg, 32, threadIdx.x & 127, 128, PP_GN_BAR + wg);
     }
     return;
   }
 
-  // ===================== consumers: two warpgroups x 64 accumulator rows =====================
-  // Accumulator fragment of m64nBNk16 (per warp 16 rows): d[4j + 2h + e] = row 16 * (warp % 4) + lane / 4 + 8h,
-  // column 8j + 2 (lane % 4) + e.
-  const int wg = warp >> 2;
+  // ===================== cooperative consumers: two warpgroups x 64 accumulator rows =====================
   const int rsub = lane >> 2, q = lane & 3;
-  const float inv_scale = __ldg(p.inv_scale);
-  const bool sliced = p.slice_kb > 0;
-  const int slice_len = sliced ? p.slice_kb : (p.kb_end - p.kb_begin);
-  float acc[NF], ext[NF];          // ext: the F8 cross products, or the running sum of the K slices
+  const uint32_t a_off = wg * (A_PLANE_BYTES / 2);  // this warpgroup's 64 rows of the A operand
+  const int slice_len = p.slice_kb > 0 ? p.slice_kb : (p.kb_end - p.kb_begin);
+  float acc[1][NF], ext[1][NF];    // ext: the F8 cross products, or the running sum of the K slices
 #pragma unroll
-  for (int i = 0; i < NF; ++i) { acc[i] = 0.f; ext[i] = 0.f; }
-  int stage = 0; uint32_t phase = 0;
-  uint32_t ncol = 0;                     // COLS: column boxes consumed (the column ring's position)
+  for (int i = 0; i < NF; ++i) { acc[0][i] = 0.f; ext[0][i] = 0.f; }
   // VQ state: the running top-4 of this thread's two rows
   float td[2][4];
   int tj[2][4];
   float a_row[2] = {0.f, 0.f};
 
-  for (int it = 0, work; (work = work_of(it)) >= 0; ++it) {
-    const TileCoord tc = decode(work);
-    // ---------------- main loop
+  for (int it = 0, work; (work = work_of<VQ>(p, it)) >= 0; ++it) {
+    const TileCoord tc = decode_tile(p, work);
     bool have_ext = F8;
-    if constexpr (COLS) {
-      // same wgmmas per k-block as below (e4m3 cross term, then hi * hi); the A operand of tap dy starts 8 (dy + 1)
-      // rows into the column box, and the box is released after its third tap
-      uint32_t more = 0;
-      for (int col = 0; col < 3 * p.cchunks; ++col, ++ncol) {        // (chunk, dx) in that order
-        const int cs = ncol % COL_STAGES;
-        mbar_wait(col_full_bar(cs), (ncol / COL_STAGES) & 1u);
-        const uint32_t ca = smem_base + cs * COL_STAGE_BYTES + wg * (A_PLANE_BYTES / 2);
-#pragma unroll 1
-        for (int dy = 0; dy < 3; ++dy) {
-          mbar_wait(full_bar(stage), phase);
-          const uint32_t sb = ring_base + stage * Cfg::STAGE_BYTES;
-          const uint64_t a_hi = make_sw128_desc(ca + 1024 * dy);
-          const uint64_t a_lo = make_sw128_desc(ca + COL_PLANE_BYTES + 1024 * dy);
-          const uint64_t b_hi = make_sw128_desc(sb);
-          const uint64_t b_lo = make_sw128_desc(sb + Cfg::B_PLANE_BYTES);
-          fence_regs(acc); fence_regs(ext);
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k) {
-            const uint64_t ko = (uint64_t)((k * 32) >> 4);
-            Wgmma<BN>::e4m3(ext, a_lo + ko, b_lo + ko, k ? 1u : more);
-            Wgmma<BN>::f16(acc, a_hi + ko, b_hi + ko, k ? 1u : more);
-          }
-          wgmma_commit();
-          wgmma_wait_all();
-          fence_regs(acc); fence_regs(ext);
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-          more = 1u;
-        }
-        if (lane == 0) mbar_arrive(col_empty_bar(cs));
+    // no k-block stays in flight: the stage (and a column box after its third tap) is released right away
+    auto kblock = [&](uint32_t a_hi, uint32_t a_lo, uint32_t b, uint32_t more, int stage, int col) {
+      mma_kblock<BN, F8, 1, 0>(acc, ext, a_hi + a_off, a_lo + a_off, b, more);
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(r.empty(stage));                 // this warp's reads of the stage are complete
+        if (col >= 0) mbar_arrive(r.col_empty(col));
       }
-    } else {
-      for (int kb0 = p.kb_begin; kb0 < p.kb_end; kb0 += slice_len) {
-        const int kb1 = min(kb0 + slice_len, p.kb_end);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint64_t a_hi = make_sw128_desc(sa + wg * (A_PLANE_BYTES / 2));
-          const uint64_t a_lo = make_sw128_desc(sa + A_PLANE_BYTES + wg * (A_PLANE_BYTES / 2));
-          const uint64_t b_hi = make_sw128_desc(sa + 2 * A_PLANE_BYTES);
-          const uint64_t b_lo = make_sw128_desc(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES);
-          fence_regs(acc); fence_regs(ext);
-          wgmma_fence();
+    };
+    auto fold = [&] {                                // sliced: fold the finished partial into the running sum
 #pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k) {
-            const uint64_t ko = (uint64_t)((k * 32) >> 4);   // +32 bytes per k-step inside the 128B swizzle atom
-            const uint32_t more = (kb != kb0 || k != 0) ? 1u : 0u;
-            // small cross terms first, the dominant hi*hi product last
-            if constexpr (F8) {
-              Wgmma<BN>::e4m3(ext, a_lo + ko, b_lo + ko, more);     // sum a_lo8 w_hi8 + sum a_hi8 w_lo8
-              Wgmma<BN>::f16(acc, a_hi + ko, b_hi + ko, more);
-            } else {
-              Wgmma<BN>::f16(acc, a_lo + ko, b_hi + ko, more);
-              Wgmma<BN>::f16(acc, a_hi + ko, b_lo + ko, 1u);
-              Wgmma<BN>::f16(acc, a_hi + ko, b_hi + ko, 1u);
-            }
-          }
-          wgmma_commit();
-          wgmma_wait_all();
-          fence_regs(acc); fence_regs(ext);
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty_bar(stage));     // this warp's reads of the stage are complete
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        if (kb1 < p.kb_end) {           // sliced: fold the finished partial into the running sum
-#pragma unroll
-          for (int i = 0; i < NF; ++i) ext[i] = have_ext ? acc[i] + ext[i] : acc[i];
-          have_ext = true;
-        }
-      }
-    }
+      for (int i = 0; i < NF; ++i) ext[0][i] = have_ext ? acc[0][i] + ext[0][i] : acc[0][i];
+      have_ext = true;
+    };
+    if constexpr (COLS) walk_columns(p, r, pos, kblock);
+    else walk_taps<true>(p, r, pos, slice_len, kblock, fold);
     if (have_ext) {
 #pragma unroll
-      for (int i = 0; i < NF; ++i) acc[i] += ext[i];
+      for (int i = 0; i < NF; ++i) acc[0][i] += ext[0][i];
     }
 
     if constexpr (VQ) {
@@ -695,7 +702,7 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
         for (int h = 0; h < 2; ++h)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const float c = acc[4 * j + 2 * h + e] * inv_scale;                                   // exact (power of two)
+            const float c = acc[0][4 * j + 2 * h + e] * inv_scale;                                // exact (power of two)
             const float d = __fsub_rn(__fadd_rn(a_row[h], e ? es.y : es.x), __fmul_rn(2.0f, c));   // fl(fl(A + B_j) - 2 C_j)
             if (d < td[h][3]) top4_insert(td[h], tj[h], d, col + e);
           }
@@ -721,72 +728,9 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
       }
       continue;
     }
-
-    // ===================== epilogue: acc * 2^-s + bias -> GELU | ReLU -> + res1 + res2 -> store =====================
-    const int Ho = p.up ? 2 * p.H : p.H, Wo = p.up ? 2 * p.W : p.W;
-    long off[2];                                         // output element offset of this thread's two rows (-1: outside)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = wg * 64 + (warp & 3) * 16 + rsub + 8 * h;
-      const int y = tc.ty * p.Ht + (row >> p.wt_shift), x = tc.tx * p.Wt + (row & (p.Wt - 1));
-      const int oy = p.up ? 2 * y + (tc.ph >> 1) : y, ox = p.up ? 2 * x + (tc.ph & 1) : x;
-      off[h] = (y < p.H && x < p.W) ? (((long)tc.b * Ho + oy) * Wo + ox) * p.Cout : -1;
-    }
-    const int gpl = BN / p.cpg;                           // GroupNorm groups of this n-tile
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int col = tc.nt * BN + 8 * j + 2 * q;
-      const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
-      float gs = 0.f, gss = 0.f;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float2 o;
-        o.x = fmaf(acc[4 * j + 2 * h], inv_scale, bb.x);     // acc * 2^-s is exact: == (acc * inv) + bias
-        o.y = fmaf(acc[4 * j + 2 * h + 1], inv_scale, bb.y);
-        if (p.act == FEMASR_ACT_GELU) { o.x = gelu_erf_fast_f(o.x); o.y = gelu_erf_fast_f(o.y); }
-        else if (p.act == FEMASR_ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
-        else if (EXT == 1 && p.act == FEMASR_ACT_LRELU) { o.x = lrelu02_f(o.x); o.y = lrelu02_f(o.y); }
-        if (off[h] >= 0) {
-          const long o_off = off[h] + col;
-          if (RES) { const float2 r = *reinterpret_cast<const float2*>(p.res1 + o_off); o.x += r.x; o.y += r.y; }
-          if (p.res2) { const float2 r = *reinterpret_cast<const float2*>(p.res2 + o_off); o.x += r.x; o.y += r.y; }
-          if (p.out_hi) {
-            uint32_t hh, ll;
-            split_pack2(o.x, o.y, hh, ll);
-            *reinterpret_cast<uint32_t*>(p.out_hi + o_off) = hh;
-            *reinterpret_cast<uint32_t*>(p.out_lo + o_off) = ll;
-          } else {
-            *reinterpret_cast<float2*>(p.y + o_off) = o;
-          }
-          gs += o.x + o.y; gss = fmaf(o.x, o.x, fmaf(o.y, o.y, gss));
-        }
-      }
-      if (p.gn_partial) {
-        // fixed-order reduction over the warp's 16 rows (lanes sharing q), then over the lanes of one group
-#pragma unroll
-        for (int o = 4; o <= 16; o <<= 1) { gs += __shfl_xor_sync(0xffffffffu, gs, o); gss += __shfl_xor_sync(0xffffffffu, gss, o); }
-        if (p.cpg >= 4) { gs += __shfl_xor_sync(0xffffffffu, gs, 1); gss += __shfl_xor_sync(0xffffffffu, gss, 1); }
-        if (p.cpg >= 8) { gs += __shfl_xor_sync(0xffffffffu, gs, 2); gss += __shfl_xor_sync(0xffffffffu, gss, 2); }
-        if (rsub == 0 && (q & (p.cpg / 2 - 1)) == 0) {
-          const int g = (8 * j + 2 * q) / p.cpg;
-          red[(warp * 64 + g) * 2] = gs;
-          red[(warp * 64 + g) * 2 + 1] = gss;
-        }
-      }
-    }
-    if (p.gn_partial) {
-      // one partial row per 32-row quarter of the tile (= the two warps of 16 rows that cover it)
-      asm volatile("bar.sync 1, %0;" ::"r"(32 * TC_CONSUMER_WARPS) : "memory");
-      const int tile_in_img = (tc.ph * p.tiles_y + tc.ty) * p.tiles_x + tc.tx;
-      for (int i = threadIdx.x; i < 4 * gpl; i += 32 * TC_CONSUMER_WARPS) {
-        const int quarter = i / gpl, g = i - quarter * gpl;
-        const float* r0 = red + ((2 * quarter) * 64 + g) * 2;
-        const float* r1 = red + ((2 * quarter + 1) * 64 + g) * 2;
-        float* gp = p.gn_partial + (((long)tc.b * p.gn_rows + tile_in_img * 4 + quarter) * 32 + tc.nt * gpl + g) * 2;
-        *reinterpret_cast<float2*>(gp) = make_float2(r0[0] + r1[0], r0[1] + r1[1]);
-      }
-      asm volatile("bar.sync 1, %0;" ::"r"(32 * TC_CONSUMER_WARPS) : "memory");
-    }
+    // 16-row group `warp` of the tile
+    epilogue_rows<BN, RES, EXT, false>(p, tc, acc[0], warp * 16, inv_scale, red, warp * 64, lane);
+    if (p.gn_partial) gn_store_partials<BN>(p, tc, red, 64, threadIdx.x, 32 * TC_CONSUMER_WARPS, TC_GN_BAR);
   }
 }
 
@@ -1178,9 +1122,26 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
+// The four operand maps of a launch: A = the NHWC fp16 planes [B][H][W][C] in 4-D boxes of 64 ch x box_w x box_h x 1,
+// traversed with the spatial stride `stride`; B = the K-major weight planes [rows][K] in 2-D boxes of 64 x BN.
+struct TcMaps { CUtensorMap a_hi, a_lo, b_hi, b_lo; };
+static int make_maps(TcMaps* m, const void* a_hi, const void* a_lo, int B, int H, int W, int C, int box_w, int box_h,
+                     int stride, const void* w_hi, const void* w_lo, long rows, long K, int BN) {
+  const cuuint64_t adims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+  const cuuint64_t astr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  const cuuint32_t abox[4] = {64, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  const cuuint64_t bdims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
+  const cuuint64_t bstr[1] = {(cuuint64_t)K * 2};
+  const cuuint32_t bbox[2] = {64, (cuuint32_t)BN};
+  int s = make_map(&m->a_hi, a_hi, 4, adims, astr, abox, stride);
+  if (!s) s = make_map(&m->a_lo, a_lo, 4, adims, astr, abox, stride);
+  if (!s) s = make_map(&m->b_hi, w_hi, 2, bdims, bstr, bbox);
+  if (!s) s = make_map(&m->b_lo, w_lo, 2, bdims, bstr, bbox);
+  return s;
+}
+
 template <int BN, bool RES, bool F8, bool VQ, int EXT = 0, bool COLS = false, bool PP = false>
-static int launch_tc_v(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
-                       const TcP& p, cudaStream_t st) {
+static int launch_tc_v(const TcMaps& m, const TcP& p, cudaStream_t st) {
   using Cfg = TcCfg<BN, COLS>;
   static PerDeviceFlag attr_set;      // per template instantiation AND per device
   if (!attr_set.cur()) {
@@ -1189,22 +1150,26 @@ static int launch_tc_v(const CUtensorMap& ah, const CUtensorMap& al, const CUten
   }
   const int items = VQ ? p.num_tiles / p.n_tiles : p.num_tiles;     // VQ: one CTA walks all code tiles of an m-tile
   const int grid = items < sm_count() ? items : sm_count();
-  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP>, dim3(grid), dim3(PP ? TC_PP_THREADS : TC_THREADS), Cfg::SMEM_BYTES, st, ah, al, bh, bl, p));
+  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP>, dim3(grid), dim3(PP ? TC_PP_THREADS : TC_THREADS),
+                         Cfg::SMEM_BYTES, st, m.a_hi, m.a_lo, m.b_hi, m.b_lo, p));
   return launch_status(VQ ? "tc_igemm_kernel(vq)" : "tc_igemm_kernel");
 }
 
-// PP: the ping-pong schedule (plan_tiles decides)
-template <int BN, bool PP = false>
-static int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
-                     const TcP& p, bool cols, cudaStream_t st) {
-  if (cols)
-    return p.res1 ? launch_tc_v<BN, true, true, false, 0, true, PP>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, true, false, 0, true, PP>(ah, al, bh, bl, p, st);
-  if (p.f8) return p.res1 ? launch_tc_v<BN, true, true, false, 0, false, PP>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, true, false, 0, false, PP>(ah, al, bh, bl, p, st);
-  if (p.taps == 25)
-    return p.res1 ? launch_tc_v<BN, true, false, false, 2, false, PP>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false, 2, false, PP>(ah, al, bh, bl, p, st);
-  if (p.taps == 16 || p.act == FEMASR_ACT_LRELU)
-    return p.res1 ? launch_tc_v<BN, true, false, false, 1, false, PP>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false, 1, false, PP>(ah, al, bh, bl, p, st);
-  return p.res1 ? launch_tc_v<BN, true, false, false, 0, false, PP>(ah, al, bh, bl, p, st) : launch_tc_v<BN, false, false, false, 0, false, PP>(ah, al, bh, bl, p, st);
+// The instantiation of a conv / linear launch: tile width BN and schedule (COLS, PP) as plan_tiles chose, then the
+// operand mode (F8), the taps / epilogue extension (EXT) and the residual (RES).  The column schedule is F8-only, and F8
+// has no 4x4 / 5x5 taps or LeakyReLU (femasr_tc_igemm refuses them), so those run with EXT = 0.
+template <int BN, bool PP, bool COLS, bool F8, int EXT>
+static int launch_tc(const TcMaps& m, const TcP& p, cudaStream_t st) {
+  return p.res1 ? launch_tc_v<BN, true, F8, false, EXT, COLS, PP>(m, p, st)
+                : launch_tc_v<BN, false, F8, false, EXT, COLS, PP>(m, p, st);
+}
+template <int BN, bool PP>
+static int launch_tc(const TcMaps& m, const TcP& p, bool cols, cudaStream_t st) {
+  if (cols) return launch_tc<BN, PP, true, true, 0>(m, p, st);
+  if (p.f8) return launch_tc<BN, PP, false, true, 0>(m, p, st);
+  if (p.taps == 25) return launch_tc<BN, PP, false, false, 2>(m, p, st);
+  if (p.taps == 16 || p.act == FEMASR_ACT_LRELU) return launch_tc<BN, PP, false, false, 1>(m, p, st);
+  return launch_tc<BN, PP, false, false, 0>(m, p, st);
 }
 
 }  // namespace femasr
@@ -1419,28 +1384,12 @@ extern "C" int femasr_vq_match_tc(const void* z_hi, const void* z_lo, const void
   p.n_tiles = n_e / BN;
   p.num_tiles = p.tiles_x * p.n_tiles; p.cchunks = e_dim / 64;
   p.kb_begin = 0; p.kb_end = p.cchunks; p.cpg = 1;
-  CUtensorMap mah, mal, mbh, mbl;
-  {
-    const cuuint64_t dims[4] = {(cuuint64_t)e_dim, (cuuint64_t)N, 1, 1};
-    const cuuint64_t str[3] = {(cuuint64_t)e_dim * 2, (cuuint64_t)N * e_dim * 2, (cuuint64_t)N * e_dim * 2};
-    const cuuint32_t box[4] = {64, 128, 1, 1};
-    int s = make_map(&mah, z_hi, 4, dims, str, box);
-    if (s) return s;
-    s = make_map(&mal, z_lo, 4, dims, str, box);
-    if (s) return s;
-  }
-  {
-    const cuuint64_t dims[2] = {(cuuint64_t)e_dim, (cuuint64_t)n_e};
-    const cuuint64_t str[1] = {(cuuint64_t)e_dim * 2};
-    const cuuint32_t box[2] = {64, (cuuint32_t)BN};
-    int s = make_map(&mbh, w_hi, 2, dims, str, box);
-    if (s) return s;
-    s = make_map(&mbl, w_lo, 2, dims, str, box);
-    if (s) return s;
-  }
+  TcMaps m;
+  const int s = make_maps(&m, z_hi, z_lo, 1, 1, N, e_dim, 128, 1, 1, w_hi, w_lo, n_e, e_dim, BN);
+  if (s) return s;
   cudaStream_t st = as_stream(stream);
-  if (BN == 128) return launch_tc_v<128, false, false, true>(mah, mal, mbh, mbl, p, st);
-  return launch_tc_v<64, false, false, true>(mah, mal, mbh, mbl, p, st);
+  if (BN == 128) return launch_tc_v<128, false, false, true>(m, p, st);
+  return launch_tc_v<64, false, false, true>(m, p, st);
 }
 
 // y = act(conv(a) + bias) + res1 + res2 with a given as fp16 hi/lo planes at the conv-input resolution.
@@ -1500,28 +1449,13 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
   FEMASR_CHECK_ARG(ntile < (1l << 31), "tc_igemm: too many tiles");
   p.num_tiles = (int)ntile; p.cchunks = a->Cin / 64;
 
-  CUtensorMap mah, mal, mbh, mbl;
-  {
-    const cuuint64_t dims[4] = {(cuuint64_t)a->Cin, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B};
-    const cuuint64_t str[3] = {(cuuint64_t)a->Cin * 2, (cuuint64_t)Win * a->Cin * 2, (cuuint64_t)Hin * Win * a->Cin * 2};
-    // with a traversal stride s the box spans s*Wt x s*Ht source pixels and lands Wt x Ht of them in smem
-    // column schedule: the box spans the tile's 16 rows plus the rows above and below
-    const cuuint32_t box[4] = {64, (cuuint32_t)(p.Wt * stride), (cuuint32_t)(plan.cols ? COL_HT + 2 : p.Ht * stride), 1};
-    int s = make_map(&mah, a->a_hi, 4, dims, str, box, stride);
-    if (s) return s;
-    s = make_map(&mal, a->a_lo, 4, dims, str, box, stride);
-    if (s) return s;
-  }
-  {
-    const cuuint64_t dims[2] = {(cuuint64_t)Ktot, (cuuint64_t)phases * a->Cout};
-    const cuuint64_t str[1] = {(cuuint64_t)Ktot * 2};
-    const cuuint32_t box[2] = {64, (cuuint32_t)BN};
-    int s = make_map(&mbh, w_hi, 2, dims, str, box);
-    if (s) return s;
-    s = make_map(&mbl, w_lo, 2, dims, str, box);
-    if (s) return s;
-  }
+  // with a traversal stride s the box spans s*Wt x s*Ht source pixels and lands Wt x Ht of them in smem; column schedule:
+  // the box spans the tile's 16 rows plus the rows above and below
+  TcMaps m;
+  const int s = make_maps(&m, a->a_hi, a->a_lo, B, Hin, Win, a->Cin, p.Wt * stride, plan.cols ? COL_HT + 2 : p.Ht * stride,
+                          stride, w_hi, w_lo, (long)phases * a->Cout, Ktot, BN);
+  if (s) return s;
   cudaStream_t st = as_stream(stream);
-  if (BN == 128) return launch_tc<128>(mah, mal, mbh, mbl, p, plan.cols, st);
-  return plan.pingpong ? launch_tc<64, true>(mah, mal, mbh, mbl, p, plan.cols, st) : launch_tc<64, false>(mah, mal, mbh, mbl, p, plan.cols, st);
+  if (BN == 128) return launch_tc<128, false>(m, p, plan.cols, st);
+  return plan.pingpong ? launch_tc<64, true>(m, p, plan.cols, st) : launch_tc<64, false>(m, p, plan.cols, st);
 }
