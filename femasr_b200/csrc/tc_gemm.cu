@@ -17,6 +17,8 @@
 //              (*2^-s + bias -> GELU -> + residual(s) -> fp32 NHWC or split-fp16 planes, GroupNorm partials, VQ top-4).
 // The ping-pong schedule (PP, 384 threads) gives the producer a warpgroup of its own and each consumer warpgroup whole
 // tiles, in turns on the tensor cores, so that one tile's epilogue runs under the next tile's MMAs.
+// The TMA epilogue (TMAE) of the cooperative BN-128 linears passes each finished tile through shared memory to TMA stores,
+// with the residual loaded by TMA, so that the consumers never wait on global memory.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
@@ -77,6 +79,26 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
+
+// TMA stores (bulk groups) of the TMA epilogue: shared -> global, clipped to the tensor's bounds
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every committed store has finished reading its shared-memory source (the box may be rewritten)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every committed store has completed (its writes are done)
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// orders this thread's generic-proxy shared-memory writes before a later TMA (async-proxy) read of them
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ float2 lds_f2(uint32_t a) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ void sts_f2(uint32_t a, float2 v) { asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v.x), "f"(v.y)); }
+__device__ __forceinline__ void sts_u32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v)); }
 
 // Programmatic dependent launch: a kernel launched with the programmatic-serialisation attribute may start (its CTAs
 // become resident as the predecessor's retire, it runs its prologue) before the predecessor has finished;
@@ -193,7 +215,7 @@ constexpr int TC_CONSUMER_WARPS = 8, TC_THREADS = 32 * TC_CONSUMER_WARPS + 32;
 // registers to the consumers: 128 x 40 + 256 x 232 = 64512 <= 65536, the 168 per thread of the launch.
 constexpr int TC_PP_THREADS = 32 * TC_CONSUMER_WARPS + 128;
 constexpr int PP_PRODUCER_REGS = 40, PP_CONSUMER_REGS = 232;
-constexpr int TC_GN_BAR = 1, PP_GN_BAR = 2, PP_ORDER_BAR = 4;   // named barriers (PP: + warpgroup)
+constexpr int TC_GN_BAR = 1, PP_GN_BAR = 2, TC_EPI_BAR = 3, PP_ORDER_BAR = 4;   // named barriers (PP: + warpgroup)
 constexpr int TC_SMEM_LIMIT = 232448;              // 227 KB of opt-in shared memory per block on H100
 
 // Column schedule (COLS): 8 x 16 output tiles; one activation box of 64 ch x 8 cols x 18 rows per (channel chunk, dx)
@@ -203,24 +225,31 @@ constexpr int COL_WT = 8, COL_HT = 16;
 constexpr int COL_PLANE_BYTES = (COL_HT + 2) * COL_WT * TC_BK * 2;   // 18 KB
 constexpr int COL_STAGE_BYTES = 2 * COL_PLANE_BYTES;                 // a_hi, a_lo8
 
-// Shared memory: [COLS: activation column ring][stage ring][barriers][GroupNorm partials].  Without COLS a stage holds
-// all four operand boxes of a k-block; with COLS it holds the two weight boxes and the activation columns have a ring of
-// their own.
-template <int BN, bool COLS = false>
+// TMA epilogue (TMAE): a 128 x 128 output tile leaves in four column blocks of 32, each through one 16 KB box of 128
+// rows x 128 bytes (fp32: 32 floats, 128B swizzle; split: 32 halves of the hi plane, then of the lo plane, 64B swizzle
+// each); two boxes alternate.
+constexpr int EPI_COLS = 32, EPI_BOX_BYTES = TC_BM * 128, EPI_BOXES = 2;
+
+// Shared memory: [COLS: activation column ring][stage ring][TMAE: epilogue boxes][barriers][GroupNorm partials].
+// Without COLS a stage holds all four operand boxes of a k-block; with COLS it holds the two weight boxes and the
+// activation columns have a ring of their own.  The TMA epilogue runs no GroupNorm partials: its boxes take their place
+// and it keeps 3 stages at BN 128 (3 x 65536 + 32768 + 1024 + 256 = 230656 bytes).
+template <int BN, bool COLS = false, bool TMAE = false>
 struct TcCfg {
   static_assert(BN == 64 || BN == 128, "tile width");
   static constexpr int B_PLANE_BYTES = BN * TC_BK * 2;
   static constexpr int STAGE_BYTES = (COLS ? 0 : 2 * A_PLANE_BYTES) + 2 * B_PLANE_BYTES;   // (a_hi, a_lo,) w_hi, w_lo
   static constexpr int COL_STAGES = COLS ? 2 : 0;
   static constexpr int COL_RING_BYTES = COL_STAGES * COL_STAGE_BYTES;
-  static constexpr int RED_BYTES = TC_CONSUMER_WARPS * 64 * 2 * 4;                  // per-warp GroupNorm partials
-  // 3 (BN 128) / 4 (BN 64); COLS: 4 (BN 128) / 9 (BN 64)
-  static constexpr int STAGES = (TC_SMEM_LIMIT - 1024 - 256 - RED_BYTES - COL_RING_BYTES) / STAGE_BYTES;
-  static constexpr int RING_BYTES = COL_RING_BYTES + STAGES * STAGE_BYTES;
+  static constexpr int RED_BYTES = TMAE ? 0 : TC_CONSUMER_WARPS * 64 * 2 * 4;       // per-warp GroupNorm partials
+  static constexpr int EPI_BYTES = TMAE ? EPI_BOXES * EPI_BOX_BYTES : 0;
+  // 3 (BN 128) / 4 (BN 64); COLS: 4 (BN 128) / 9 (BN 64); TMAE: 3
+  static constexpr int STAGES = (TC_SMEM_LIMIT - 1024 - 256 - RED_BYTES - COL_RING_BYTES - EPI_BYTES) / STAGE_BYTES;
+  static constexpr int RING_BYTES = COL_RING_BYTES + STAGES * STAGE_BYTES + EPI_BYTES;
   static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + RED_BYTES;
   static constexpr int NF = BN / 2;                                                  // accumulator floats per thread
   static_assert(SMEM_BYTES <= TC_SMEM_LIMIT, "shared memory budget");
-  static_assert(16 * (STAGES + COL_STAGES) <= 256, "barrier area");
+  static_assert(16 * (STAGES + COL_STAGES) + 8 * (TMAE ? EPI_BOXES : 0) <= 256, "barrier area");
 };
 
 // running top-4 of (d, j), ascending lexicographically; precondition: (d, j) sorts before (td[3], tj[3])
@@ -268,6 +297,9 @@ struct Rings {
   __device__ __forceinline__ uint32_t empty(int s) const { return bar_base + 8u * (Cfg::STAGES + s); }
   __device__ __forceinline__ uint32_t col_full(int s) const { return bar_base + 8u * (2 * Cfg::STAGES + s); }
   __device__ __forceinline__ uint32_t col_empty(int s) const { return bar_base + 8u * (2 * Cfg::STAGES + Cfg::COL_STAGES + s); }
+  // TMAE: epilogue box b and the barrier its residual block's TMA load completes on
+  __device__ __forceinline__ uint32_t epi(int b) const { return smem_base + Cfg::RING_BYTES - Cfg::EPI_BYTES + b * EPI_BOX_BYTES; }
+  __device__ __forceinline__ uint32_t epi_full(int b) const { return bar_base + 8u * (2 * Cfg::STAGES + 2 * Cfg::COL_STAGES + b); }
 };
 
 // ---------------------------------------------------------------- TMA producer (one elected lane)
@@ -525,6 +557,100 @@ __device__ __forceinline__ void gn_store_partials(const TcP& p, const TileCoord&
   named_bar_sync(bar, nthreads);
 }
 
+// ---------------------------------------------------------------- TMA epilogue (TMAE: cooperative BN-128 linears)
+// The output (fp32 y, or the hi and lo planes) and residual tensor maps: 2-D [tokens][Cout], boxes of 32 columns x 128
+// rows (tc_tma_epi_maps)
+struct EpiMaps { const CUtensorMap *out0, *out1, *res; };
+
+// Residual column block s (columns 32 s .. 32 s + 31 of the tile) of tile tc into box s % 2 by TMA, completing on that
+// box's epi_full barrier.  Rows past the last token arrive as zeros and are never stored.
+template <class Cfg>
+__device__ __forceinline__ void load_res_block(const TcP& p, const Rings<Cfg>& r, const EpiMaps& e, const TileCoord& tc,
+                                               int s) {
+  const int b = s & 1;
+  mbar_expect_tx(r.epi_full(b), EPI_BOX_BYTES);
+  tma_load_2d(r.epi(b), e.res, r.epi_full(b), tc.nt * 128 + EPI_COLS * s, tc.tx * p.Wt);
+}
+
+// The same rule per element as epilogue_rows (acc * 2^-s + bias -> GELU | ReLU -> + res1 -> fp32 or split_pack2), but
+// the tile leaves through shared memory: for each column block s = 0..3 the 256 consumer threads write box s % 2, meet
+// at TC_EPI_BAR, and thread 0 stores the box by TMA (bulk group) and goes on; the consumers never wait for global memory.
+// Box reuse: before each barrier thread 0 waits until the previous block's store has read its box, so after the barrier
+// the other box is free.  RES: block s's residual is already in box s % 2 (epi_full, parity s / 2: each box is loaded
+// twice per tile) and each thread reads its residual where it then writes its output; thread 0 loads block s + 1 as soon
+// as its box is free, and blocks 0 and 1 of the next tile (`next`) at block 3, so those load under its k-loop (the first
+// tile's: before the tile loop).  A tile's residual is read before that tile is stored, so y == res1 is safe.
+// Bank conflicts: the split planes' 4-byte stores cover all 32 banks per warp.  The fp32 8-byte accesses are 2-way
+// conflicted (a half-warp spans 4 rows, so the swizzle spreads it over only 4 of the 8 chunks); permuting the column
+// blocks across lanes to avoid that costs the residual kernel spills at 168 registers.
+template <bool RES, class Cfg>
+__device__ __forceinline__ void epilogue_tma(const TcP& p, const Rings<Cfg>& r, const EpiMaps& e, const TileCoord& tc,
+                                             int next, const float (&acc)[64], float inv_scale, int warp, int lane) {
+  const int rsub = lane >> 2, q = lane & 3;
+  const int row = warp * 16 + rsub;                       // rows row and row + 8 of the tile
+  // fp32, 128B swizzle: (row, column 8 jj + 2 q) at row * 128 + (((2 jj + q / 2) ^ (row % 8)) << 4) + (q % 2) * 8,
+  // i.e. 16-byte chunk 2 jj ^ f_x
+  const uint32_t f_base = row * 128 + (q & 1) * 8;
+  const int f_x = (q >> 1) ^ (row & 7);
+  // split, 64B swizzle (per plane: 64-byte rows): row * 64 + ((jj ^ (row / 2 % 4)) << 4) + 4 q, i.e. chunk jj ^ h_x
+  const uint32_t h_base = row * 64 + 4 * q;
+  const int h_x = (row >> 1) & 3;
+  const bool split = p.out_hi != nullptr;
+  const int n0 = tc.nt * 128, row0 = tc.tx * p.Wt;
+#pragma unroll
+  for (int s = 0; s < 4; ++s) {
+    const int b = s & 1;
+    const uint32_t box = r.epi(b);
+    if (RES) mbar_wait(r.epi_full(b), (uint32_t)(s >> 1));
+    // row by row (h), so that only one row's residuals (8 registers) are live: at 168 registers more spills
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float2 res[4];
+      if constexpr (RES) {
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) res[jj] = lds_f2(box + f_base + 1024 * h + ((2 * jj ^ f_x) << 4));
+      }
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 4 * s + jj;
+        const int col = n0 + 8 * j + 2 * q;
+        const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
+        float2 o;
+        o.x = fmaf(acc[4 * j + 2 * h], inv_scale, bb.x);
+        o.y = fmaf(acc[4 * j + 2 * h + 1], inv_scale, bb.y);
+        if (p.act == FEMASR_ACT_GELU) { o.x = gelu_erf_fast_f(o.x); o.y = gelu_erf_fast_f(o.y); }
+        else if (p.act == FEMASR_ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+        if (split) {                                       // (never with RES: plan_tiles)
+          uint32_t hh, ll;
+          split_pack2(o.x, o.y, hh, ll);
+          const uint32_t a = box + h_base + 512 * h + ((jj ^ h_x) << 4);
+          sts_u32(a, hh);
+          sts_u32(a + EPI_BOX_BYTES / 2, ll);
+        } else {
+          if (RES) { o.x += res[jj].x; o.y += res[jj].y; }
+          sts_f2(box + f_base + 1024 * h + ((2 * jj ^ f_x) << 4), o);
+        }
+      }
+    }
+    fence_proxy_async_smem();
+    if (threadIdx.x == 0) {
+      bulk_wait_read_all();                               // the previous block's box (b ^ 1) is free
+      if (RES && (s == 1 || s == 2)) load_res_block(p, r, e, tc, s + 1);
+      if (RES && s == 3 && next >= 0) load_res_block(p, r, e, decode_tile(p, next), 0);
+    }
+    named_bar_sync(TC_EPI_BAR, 32 * TC_CONSUMER_WARPS);
+    if (threadIdx.x == 0) {
+      tma_store_2d(e.out0, box, n0 + EPI_COLS * s, row0);
+      if (split) tma_store_2d(e.out1, box + EPI_BOX_BYTES / 2, n0 + EPI_COLS * s, row0);
+      bulk_commit();
+      if (RES && s == 3 && next >= 0) {
+        bulk_wait_read_all();                             // box 1 read out: the next tile's block 1 loads under its k-loop
+        load_res_block(p, r, e, decode_tile(p, next), 1);
+      }
+    }
+  }
+}
+
 // RES: the layer adds a residual tile (res1) in the epilogue (a template parameter: the load is in the hot loop).
 // F8: the F8 cross-term mode (p.f8).  A template parameter because a runtime choice between the two accumulator sets
 // inside the k-loop makes ptxas serialise every wgmma of the kernel.
@@ -539,15 +665,20 @@ __device__ __forceinline__ void gn_store_partials(const TcP& p, const TileCoord&
 // the two take turns on the tensor cores, and one runs its epilogue while the other runs its k-loop (plan_tiles).
 // Both schedules issue their k-blocks through mma_kblock, walk the rings with walk_columns / walk_taps and store through
 // epilogue_rows and gn_store_partials; they differ in how many k-blocks stay in flight and where a stage is released.
-template <int BN, bool RES, bool F8, bool VQ = false, int EXT = 0, bool COLS = false, bool PP = false>
+// TMAE: the cooperative BN-128 linears (1x1, no F8, no GroupNorm partials, no res2) store through epilogue_tma and the
+// output / residual maps map_o0, map_o1, map_r (unused otherwise), instead of from registers (plan_tiles).
+template <int BN, bool RES, bool F8, bool VQ = false, int EXT = 0, bool COLS = false, bool PP = false, bool TMAE = false>
 __global__ void __launch_bounds__(PP ? TC_PP_THREADS : TC_THREADS, 1)
 tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const TcP p) {
-  using Cfg = TcCfg<BN, COLS>;
+                const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const TcP p,
+                const __grid_constant__ CUtensorMap map_o0, const __grid_constant__ CUtensorMap map_o1,
+                const __grid_constant__ CUtensorMap map_r) {
+  using Cfg = TcCfg<BN, COLS, TMAE>;
   constexpr int NF = Cfg::NF;
   static_assert(!VQ || (!RES && !F8), "VQ mode: plain linear tiles");
   static_assert(!COLS || (F8 && !VQ && EXT == 0), "column schedule: F8 3x3 convs");
   static_assert(!PP || (BN == 64 && !VQ), "ping-pong schedule: BN-64 convs and linears");
+  static_assert(!TMAE || (BN == 128 && !F8 && !VQ && EXT == 0 && !COLS && !PP), "TMA epilogue: cooperative BN-128 linears");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const Rings<Cfg> r{smem_base, smem_base + Cfg::RING_BYTES};
@@ -560,6 +691,7 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
     constexpr int READERS = PP ? TC_CONSUMER_WARPS / 2 : TC_CONSUMER_WARPS;
     for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(r.full(s), 1); mbar_init(r.empty(s), READERS); }
     for (int s = 0; s < Cfg::COL_STAGES; ++s) { mbar_init(r.col_full(s), 1); mbar_init(r.col_empty(s), READERS); }
+    if (TMAE) for (int b = 0; b < EPI_BOXES; ++b) mbar_init(r.epi_full(b), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -652,6 +784,12 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
   int tj[2][4];
   float a_row[2] = {0.f, 0.f};
 
+  if (TMAE && RES && threadIdx.x == 0 && work_of<false>(p, 0) >= 0) {
+    const TileCoord tc = decode_tile(p, work_of<false>(p, 0));     // the first tile's residual blocks 0 and 1
+    load_res_block(p, r, EpiMaps{&map_o0, &map_o1, &map_r}, tc, 0);
+    load_res_block(p, r, EpiMaps{&map_o0, &map_o1, &map_r}, tc, 1);
+  }
+
   for (int it = 0, work; (work = work_of<VQ>(p, it)) >= 0; ++it) {
     const TileCoord tc = decode_tile(p, work);
     bool have_ext = F8;
@@ -728,10 +866,15 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
       }
       continue;
     }
+    if constexpr (TMAE) {
+      epilogue_tma<RES>(p, r, EpiMaps{&map_o0, &map_o1, &map_r}, tc, work_of<false>(p, it + 1), acc[0], inv_scale, warp, lane);
+      continue;
+    }
     // 16-row group `warp` of the tile
     epilogue_rows<BN, RES, EXT, false>(p, tc, acc[0], warp * 16, inv_scale, red, warp * 64, lane);
     if (p.gn_partial) gn_store_partials<BN>(p, tc, red, 64, threadIdx.x, 32 * TC_CONSUMER_WARPS, TC_GN_BAR);
   }
+  if (TMAE && threadIdx.x == 0) bulk_wait_all();    // the tile stores complete before the CTA exits
 }
 
 // ------------------------------------------------------------------------------------------------ operand preparation
@@ -1124,7 +1267,8 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 
 // The four operand maps of a launch: A = the NHWC fp16 planes [B][H][W][C] in 4-D boxes of 64 ch x box_w x box_h x 1,
 // traversed with the spatial stride `stride`; B = the K-major weight planes [rows][K] in 2-D boxes of 64 x BN.
-struct TcMaps { CUtensorMap a_hi, a_lo, b_hi, b_lo; };
+// TMAE launches add the output and residual maps (tc_tma_epi_maps); the others pass them unset.
+struct TcMaps { CUtensorMap a_hi, a_lo, b_hi, b_lo, o0, o1, res; };
 static int make_maps(TcMaps* m, const void* a_hi, const void* a_lo, int B, int H, int W, int C, int box_w, int box_h,
                      int stride, const void* w_hi, const void* w_lo, long rows, long K, int BN) {
   const cuuint64_t adims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
@@ -1140,18 +1284,36 @@ static int make_maps(TcMaps* m, const void* a_hi, const void* a_lo, int B, int H
   return s;
 }
 
-template <int BN, bool RES, bool F8, bool VQ, int EXT = 0, bool COLS = false, bool PP = false>
+// The TMA epilogue's maps over the 1x1 launch's token row ([tokens][Cout], tokens = p.W): fp32 y (or the split hi and
+// lo planes) and res1, boxes of 32 columns x 128 rows = 128-byte rows (fp32: 128B swizzle; fp16 planes: 64-byte rows,
+// 64B swizzle), matching epilogue_tma's shared-memory layout.  The store clips the rows past the last token.
+static int tc_tma_epi_maps(TcMaps* m, const TcP& p) {
+  const cuuint64_t dims[2] = {(cuuint64_t)p.Cout, (cuuint64_t)p.W};
+  const cuuint32_t box[2] = {(cuuint32_t)EPI_COLS, (cuuint32_t)TC_BM};
+  const cuuint64_t str32[1] = {(cuuint64_t)p.Cout * 4}, str16[1] = {(cuuint64_t)p.Cout * 2};
+  int s = FEMASR_OK;
+  if (p.out_hi) {
+    s = make_map(&m->o0, p.out_hi, 2, dims, str16, box, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, CU_TENSOR_MAP_SWIZZLE_64B);
+    if (!s) s = make_map(&m->o1, p.out_lo, 2, dims, str16, box, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, CU_TENSOR_MAP_SWIZZLE_64B);
+  } else {
+    s = make_map(&m->o0, p.y, 2, dims, str32, box, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
+  }
+  if (!s && p.res1) s = make_map(&m->res, p.res1, 2, dims, str32, box, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
+  return s;
+}
+
+template <int BN, bool RES, bool F8, bool VQ, int EXT = 0, bool COLS = false, bool PP = false, bool TMAE = false>
 static int launch_tc_v(const TcMaps& m, const TcP& p, cudaStream_t st) {
-  using Cfg = TcCfg<BN, COLS>;
+  using Cfg = TcCfg<BN, COLS, TMAE>;
   static PerDeviceFlag attr_set;      // per template instantiation AND per device
   if (!attr_set.cur()) {
-    FEMASR_CUDA(cudaFuncSetAttribute(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    FEMASR_CUDA(cudaFuncSetAttribute(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP, TMAE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set.cur() = true;
   }
   const int items = VQ ? p.num_tiles / p.n_tiles : p.num_tiles;     // VQ: one CTA walks all code tiles of an m-tile
   const int grid = items < sm_count() ? items : sm_count();
-  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP>, dim3(grid), dim3(PP ? TC_PP_THREADS : TC_THREADS),
-                         Cfg::SMEM_BYTES, st, m.a_hi, m.a_lo, m.b_hi, m.b_lo, p));
+  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP, TMAE>, dim3(grid), dim3(PP ? TC_PP_THREADS : TC_THREADS),
+                         Cfg::SMEM_BYTES, st, m.a_hi, m.a_lo, m.b_hi, m.b_lo, p, m.o0, m.o1, m.res));
   return launch_status(VQ ? "tc_igemm_kernel(vq)" : "tc_igemm_kernel");
 }
 
@@ -1199,10 +1361,15 @@ static void tc_tile_shape(int H, int W, int* Wt, int* Ht) {
 // schedule: with F8 or K slicing its two accumulators do not fit in one warpgroup, and without them (the linears)
 // ping-pong measured slower on H100 - their short k-loops cannot hide an epilogue that one warpgroup runs alone.  It
 // changes neither the tiling nor any sum.  FEMASR_TC_PINGPONG=0 keeps the cooperative schedule (for A/B timing).
-struct TilePlan { int Wt, Ht, wt_shift, tiles_x, tiles_y, BN; bool cols, pingpong; };
+// The TMA epilogue (tc_igemm_kernel's TMAE) runs the cooperative BN-128 1x1 launches without F8, GroupNorm partials,
+// res2 or LeakyReLU, and without a residual beside a split output (the Swin linears, the 1x1s before the VQ, the im2col
+// first-conv GEMM at Cout 128 / 256, conv_semantic): their short k-loops left the tensor cores idle while the register
+// epilogue waited on global memory.  FEMASR_TC_TMA_EPILOGUE=0 keeps the register epilogue (for A/B timing).
+struct TilePlan { int Wt, Ht, wt_shift, tiles_x, tiles_y, BN; bool cols, pingpong, tma_epilogue; };
 static TilePlan plan_tiles(const femasr_tc_args* a, int H, int W, bool sliced = false) {
   static const int cols_env = [] { const char* e = getenv("FEMASR_TC_COLUMNS"); return e ? atoi(e) : 1; }();
   static const int pp_env = [] { const char* e = getenv("FEMASR_TC_PINGPONG"); return e ? atoi(e) : 1; }();
+  static const int tma_env = [] { const char* e = getenv("FEMASR_TC_TMA_EPILOGUE"); return e ? atoi(e) : 1; }();
   TilePlan t;
   t.BN = a->Cout % 128 == 0 ? 128 : 64;
   tc_tile_shape(H, W, &t.Wt, &t.Ht);   // the widest power-of-two Wt <= 128 that wastes the fewest padded pixels
@@ -1213,6 +1380,12 @@ static TilePlan plan_tiles(const femasr_tc_args* a, int H, int W, bool sliced = 
   if (t.cols) { t.Wt = COL_WT; t.Ht = COL_HT; t.tiles_x = (int)cdiv(W, COL_WT); t.tiles_y = (int)cdiv(H, COL_HT); }
   t.wt_shift = 0; while ((1 << t.wt_shift) < t.Wt) ++t.wt_shift;
   t.pingpong = pp_env && !sliced && t.BN == 64;
+  // 16-byte aligned outputs and residual: the TMA maps' global addresses
+  auto al16 = [](const void* q) { return ((uintptr_t)q & 15u) == 0; };
+  const bool split = a->out_hi != nullptr;
+  t.tma_epilogue = tma_env && t.BN == 128 && !t.pingpong && !t.cols && a->ksize == 1 && !a->f8 && !a->gn_partial &&
+                   !a->res2 && a->act != FEMASR_ACT_LRELU && !(split && a->res1) &&
+                   (split ? al16(a->out_hi) && al16(a->out_lo) : al16(a->y)) && (!a->res1 || al16(a->res1));
   return t;
 }
 
@@ -1384,7 +1557,7 @@ extern "C" int femasr_vq_match_tc(const void* z_hi, const void* z_lo, const void
   p.n_tiles = n_e / BN;
   p.num_tiles = p.tiles_x * p.n_tiles; p.cchunks = e_dim / 64;
   p.kb_begin = 0; p.kb_end = p.cchunks; p.cpg = 1;
-  TcMaps m;
+  TcMaps m = {};
   const int s = make_maps(&m, z_hi, z_lo, 1, 1, N, e_dim, 128, 1, 1, w_hi, w_lo, n_e, e_dim, BN);
   if (s) return s;
   cudaStream_t st = as_stream(stream);
@@ -1451,11 +1624,17 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
 
   // with a traversal stride s the box spans s*Wt x s*Ht source pixels and lands Wt x Ht of them in smem; column schedule:
   // the box spans the tile's 16 rows plus the rows above and below
-  TcMaps m;
+  TcMaps m = {};
   const int s = make_maps(&m, a->a_hi, a->a_lo, B, Hin, Win, a->Cin, p.Wt * stride, plan.cols ? COL_HT + 2 : p.Ht * stride,
                           stride, w_hi, w_lo, (long)phases * a->Cout, Ktot, BN);
   if (s) return s;
   cudaStream_t st = as_stream(stream);
+  if (plan.tma_epilogue) {
+    const int se = tc_tma_epi_maps(&m, p);
+    if (se) return se;
+    return p.res1 ? launch_tc_v<128, true, false, false, 0, false, false, true>(m, p, st)
+                  : launch_tc_v<128, false, false, false, 0, false, false, true>(m, p, st);
+  }
   if (BN == 128) return launch_tc<128, false>(m, p, plan.cols, st);
   return plan.pingpong ? launch_tc<64, true>(m, p, plan.cols, st) : launch_tc<64, false>(m, p, plan.cols, st);
 }

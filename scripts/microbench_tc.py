@@ -22,6 +22,15 @@ if os.environ.get('MB_PINGPONG') == 'ab':
         subprocess.run([sys.executable, os.path.abspath(__file__)], env=env, check=True)
     sys.exit(0)
 
+# MB_TMAEPI=ab: the linears the TMA epilogue runs (the Swin linears at the engine's geometry) with it
+# (FEMASR_TC_TMA_EPILOGUE=1) and with the register epilogue (=0)
+if os.environ.get('MB_TMAEPI') == 'ab':
+    for v in ('1', '0'):
+        print(f"# FEMASR_TC_TMA_EPILOGUE={v}", flush=True)
+        env = dict(os.environ, MB_TMAEPI='', FEMASR_TC_TMA_EPILOGUE=v, MB_ONLY=os.environ.get('MB_ONLY') or 'qkv|proj|fc1|fc2')
+        subprocess.run([sys.executable, os.path.abspath(__file__)], env=env, check=True)
+    sys.exit(0)
+
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -51,7 +60,8 @@ F8 = int(os.environ.get('MB_F8', '0'))      # 1: the 3x3 convs in the F8 cross-t
 GN = int(os.environ.get('MB_GN', '0'))      # 1: the 3x3 convs also emit GroupNorm partial sums (what most of them do in the network)
 
 
-def conv_case(name, B, H, W, Cin, Cout, ksize=3, up=0, res=False, act=0, split=False, bias=True, slice_kb=0):
+def conv_case(name, B, H, W, Cin, Cout, ksize=3, up=0, res=False, act=0, split=False, bias=True, slice_kb=0, inplace=False):
+    """inplace: the output overwrites the residual (y = res1), as proj and fc2 do in the network."""
     if ONLY and not any(o in name for o in ONLY.split('|')):
         return 0.0
     hi = (torch.randn(B, H, W, Cin, device=dev) * 0.5).half()
@@ -66,6 +76,8 @@ def conv_case(name, B, H, W, Cin, Cout, ksize=3, up=0, res=False, act=0, split=F
     u = 2 if up else 1
     y = None if split else torch.empty(B, H * u, W * u, Cout, device=dev)
     r = torch.randn(B, H * u, W * u, Cout, device=dev) if res else None
+    if inplace:
+        y = r
     gn = None
     if GN and ksize == 3 and not split:
         gn = torch.empty(B * G.tc_gn_rows(B, H, W, Cin, Cout, upsample=up, slice_kb=slice_kb, pair=PAIR, strip=STRIP) * 64, device=dev)
@@ -77,16 +89,16 @@ def conv_case(name, B, H, W, Cin, Cout, ksize=3, up=0, res=False, act=0, split=F
     return ms
 
 
-M = 32 * 64 * 64
-print("# Swin linears (tokens = 131072)")
-conv_case("qkv 256->768", 1, 1, M, 256, 768, 1)
-conv_case("proj 256->256 +res", 1, 1, M, 256, 256, 1, res=True)
-conv_case("fc1 256->1024 gelu fp32 out", 1, 1, M, 256, 1024, 1, act=1)
-conv_case("fc1 256->1024 gelu split out", 1, 1, M, 256, 1024, 1, act=1, split=True)
-conv_case("fc1 256->1024 noact fp32 out", 1, 1, M, 256, 1024, 1, act=0)
-conv_case("fc2 1024->256 +res", 1, 1, M, 1024, 256, 1, res=True)
+print("# Swin linears, batch 32 @64x64 (tokens = 131072)")
+conv_case("qkv 256->768", 32, 64, 64, 256, 768, 1)
+conv_case("proj 256->256 +res", 32, 64, 64, 256, 256, 1, res=True)
+conv_case("proj 256->256 +res in place", 32, 64, 64, 256, 256, 1, res=True, inplace=True)
+conv_case("fc1 256->1024 gelu fp32 out", 32, 64, 64, 256, 1024, 1, act=1)
+conv_case("fc1 256->1024 gelu split out", 32, 64, 64, 256, 1024, 1, act=1, split=True)
+conv_case("fc1 256->1024 noact fp32 out", 32, 64, 64, 256, 1024, 1, act=0)
+conv_case("fc2 1024->256 +res", 32, 64, 64, 1024, 256, 1, res=True)
 print("# K-sliced accumulation (layers in front of the VQ): accumulator folded into an fp32 running sum every 256 of K")
-conv_case("fc2 1024->256 +res sliced", 1, 1, M, 1024, 256, 1, res=True, slice_kb=4)
+conv_case("fc2 1024->256 +res sliced in place", 32, 64, 64, 1024, 256, 1, res=True, slice_kb=4, inplace=True)
 conv_case("conv 256->256 @64x64 +res sliced", 32, 64, 64, 256, 256, res=True, slice_kb=4)
 print("# 3x3 convs, batch 32")
 conv_case("conv 256->256 @64x64 +res", 32, 64, 64, 256, 256, res=True)
