@@ -115,6 +115,22 @@ struct DevParam {
 };
 
 struct Tap { float* dst; size_t cap; };
+struct Capture { void* dst; size_t bytes; };   // femasr_net_set_conv_capture
+
+// One Ctx::conv call as femasr_net_conv_trace_json reports it
+struct ConvRec {
+  std::string w;
+  int B, H, W, Cin, Cout, k, stride, upsample;
+  bool tc;
+  int pro, act;                  // prologue as staged (after Ctx::numerics), FEMASR_ACT_*
+  bool bias;
+  int res1;                      // 0 none, 1 its own tensor, 2 the output buffer
+  bool res2, split, gn_partial;
+  int operand;                   // 0 staged from fp32, 1 split planes a producer wrote, 2 im2col rows
+  bool semantic, sn;
+  int slice_kb;
+  bool f8, precise_region;
+};
 
 struct ProfRec { const char* name; double flops; cudaEvent_t e0, e1; };
 
@@ -133,6 +149,9 @@ struct femasr_net {
   int level_cb[3] = {0, -1, -1};          // decoder level i (resolution 32 << i) -> codebook index or -1
   int last_q_level = 0;                   // last decoder level that quantises (everything before it is index-critical)
   std::map<std::string, Tap> taps;
+  std::map<std::pair<int, std::string>, Capture> captures;   // (conv ordinal, operand name) -> destination
+  std::vector<ConvRec> trace;             // the Ctx::conv calls of the last run, sizing runs included
+  std::string trace_json;
   int last_launches = 0;
   bool profile = false;
   int poison = -1;                        // femasr_net_set_poison: byte every workspace block is filled with, -1 = off
@@ -378,6 +397,7 @@ struct Ctx {
   float* sem_loss = nullptr;     // forward_sem: the semantic loss output (non-NULL = run the VGG branch)
   float* vgg_feat = nullptr;     // relu4_4 [B,H/8,W/8,512], alive from the VGG stage to the loss at quantising level 0
   bool precise_region = false;   // true while emitting the layers in front of the VQ (index-critical)
+  std::set<std::pair<int, std::string>> captured;   // the registered conv captures this run has copied
 
   // workspace == nullptr: a sizing run (allocations and FLOPs only, nothing launched); else a run over the caller's
   // workspace, aligned up to 256 bytes
@@ -388,6 +408,7 @@ struct Ctx {
     ar.cap = ar.dry ? 0 : bytes - mis;
     ar.poison = ar.dry ? -1 : n->poison;
     ar.st = st;
+    n->trace.clear();
   }
   bool dry() const { return ar.dry; }
   bool ok() const { return status == FEMASR_OK; }
@@ -396,6 +417,10 @@ struct Ctx {
   int finish() {
     if (!dry()) net->last_launches = (int)(g_launches - l0);
     if (ar.poison_err != cudaSuccess) check(fail(FEMASR_ERR_CUDA, std::string("poison memset: ") + cudaGetErrorString(ar.poison_err)));
+    for (const auto& kv : net->captures)
+      if (ok() && !captured.count(kv.first))
+        check(fail(FEMASR_ERR_ARG, "conv capture " + std::to_string(kv.first.first) + " " + kv.first.second +
+                                       ": the run has no such conv operand"));
     return status;
   }
 
@@ -445,12 +470,39 @@ struct Ctx {
     auto it = net->taps.find(stage);
     return it != net->taps.end() && it->second.dst;
   }
+  // a stream-ordered copy of `bytes` from src into a caller's buffer of `cap` bytes (taps and conv captures)
+  void copy_out(const std::string& what, void* dst, size_t cap, const void* src, size_t bytes) {
+    if (cap < bytes) { check(fail(FEMASR_ERR_ARG, what + " buffer too small")); return; }
+    cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st);
+    if (e != cudaSuccess) check(fail(FEMASR_ERR_CUDA, cudaGetErrorString(e)));
+  }
   void tap(const char* stage, const float* src, size_t n) {
     if (dry() || !ok() || !tapped(stage)) return;
     const Tap& t = net->taps.at(stage);
-    if (t.cap < n) { check(fail(FEMASR_ERR_ARG, std::string("tap buffer too small: ") + stage)); return; }
-    cudaError_t e = cudaMemcpyAsync(t.dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
-    if (e != cudaSuccess) check(fail(FEMASR_ERR_CUDA, cudaGetErrorString(e)));
+    copy_out(std::string("tap ") + stage, t.dst, t.cap * sizeof(float), src, n * sizeof(float));
+  }
+
+  // femasr_net_set_conv_capture: the registered operands of conv `ord` (d), inputs before its launches (res1 may be the
+  // output buffer), outputs after them.  gn_floats: the size of d.gn_partial.
+  void capture(int ord, const ConvDesc& d, bool after, size_t gn_floats) {
+    if (!ok()) return;
+    const int ho = d.stride == 2 ? (d.H + 2 - d.k) / 2 + 1 : d.H << d.upsample;
+    const int wo = d.stride == 2 ? (d.W + 2 - d.k) / 2 + 1 : d.W << d.upsample;
+    const size_t in = (size_t)d.B * d.H * d.W * d.Cin, out = (size_t)d.B * ho * wo * d.Cout;
+    const size_t table = d.pro == FEMASR_PRO_LN ? (size_t)d.B * d.H * d.W : (size_t)d.B * d.Cin;   // LN mean / rstd, GN
+    struct Src { const char* what; const void* p; size_t bytes; bool after; };
+    const Src srcs[] = {{"x", d.x, in * 4, false},          {"a_hi", d.a_hi, in * 2, false}, {"a_lo", d.a_lo, in * 2, false},
+                        {"pa", d.pa, table * 4, false},     {"pb", d.pb, table * 4, false},  {"res1", d.res1, out * 4, false},
+                        {"res2", d.res2, out * 4, false},   {"y", d.y, out * 4, true},       {"o_hi", d.o_hi, out * 2, true},
+                        {"o_lo", d.o_lo, out * 2, true},    {"gn_partial", d.gn_partial, gn_floats * 4, true}};
+    for (const Src& s : srcs) {
+      if (s.after != after || !s.p) continue;
+      const auto key = std::make_pair(ord, std::string(s.what));
+      auto it = net->captures.find(key);
+      if (it == net->captures.end()) continue;
+      copy_out("conv capture " + std::to_string(ord) + " " + s.what, it->second.dst, it->second.bytes, s.p, s.bytes);
+      captured.insert(key);
+    }
   }
 
   // the wgmma implicit GEMM wherever the spec gave the weight its tensor-core form (gemm_path 1), else the SIMT one
@@ -499,7 +551,16 @@ struct Ctx {
   // plane) unless the producer already wrote split planes; a fused nearest-x2 upsample runs as four sub-pixel 2x2 convs
   // on the low-res operand.  Allocation happens in sizing runs too.
   void conv(const ConvDesc& d) {
-    if (!use_tc(d)) {
+    const bool tc = use_tc(d);
+    const Numerics m = tc ? numerics(d) : Numerics{0, false, d.pro};
+    const int ord = (int)net->trace.size();
+    net->trace.push_back(ConvRec{d.wname(), d.B, d.H, d.W, d.Cin, d.Cout, d.k, d.stride, d.upsample, tc, m.prologue, d.act,
+                                 d.bias, !d.res1 ? 0 : d.res1 == d.y ? 2 : 1, d.res2 != nullptr, d.o_hi != nullptr,
+                                 d.gn_partial != nullptr, d.im2col ? 2 : d.a_hi ? 1 : 0, d.semantic, d.sn, m.slice_kb,
+                                 m.f8, precise_region});
+    const bool cap = !net->captures.empty() && !dry();
+    if (cap) capture(ord, d, false, 0);
+    if (!tc) {
       femasr_igemm_args a;
       memset(&a, 0, sizeof(a));
       a.x = d.x; a.w = static_cast<const float*>(weight(d, false, false)); a.bias = d.bias ? P(d.w + ".bias") : nullptr;
@@ -507,9 +568,9 @@ struct Ctx {
       a.B = d.B; a.Hin = d.H; a.Win = d.W; a.Cin = d.Cin; a.Cout = d.Cout; a.ksize = d.k; a.stride = d.stride;
       a.upsample = d.upsample; a.prologue = d.pro; a.act = d.act;
       run(d.name ? d.name : "igemm_simt", conv_flops(d), [&] { return femasr_igemm_simt(&a, st); });
+      if (cap) capture(ord, d, true, 0);
       return;
     }
-    const Numerics m = numerics(d);
     float *ahi = nullptr, *alo = nullptr;
     if (!d.a_hi) {
       const size_t plane_halves = (size_t)d.B * d.H * d.W * d.Cin;
@@ -524,6 +585,7 @@ struct Ctx {
     const femasr_tc_args t = tc_args(d, m, ahi ? ahi : d.a_hi, ahi ? alo : d.a_lo);
     run(d.name ? d.name : detail_name("tc_igemm", d.k, d.Cin, d.Cout, d.H, d.W, d.upsample, d.stride, t.slice_kb),
         conv_flops(d), [&] { return femasr_tc_igemm(&t, st); });
+    if (cap) capture(ord, d, true, d.gn_partial ? (size_t)d.B * femasr_tc_gn_partial_rows(&t) * 32 * 2 : 0);
     if (alo) ar.release(alo);
     if (ahi) ar.release(ahi);
   }
@@ -1380,6 +1442,42 @@ extern "C" int femasr_net_set_tap(femasr_net* net, const char* stage, float* dst
   if (dst) net->taps[stage] = Tap{dst, capacity};
   else net->taps.erase(stage);
   return FEMASR_OK;
+}
+
+extern "C" int femasr_net_set_conv_capture(femasr_net* net, int ordinal, const char* what, void* dst, size_t bytes) {
+  FEMASR_CHECK_ARG(net && what, "set_conv_capture: null pointer");
+  FEMASR_CHECK_ARG(ordinal >= 0, "set_conv_capture: negative ordinal");
+  static const char* names[] = {"x", "a_hi", "a_lo", "pa", "pb", "res1", "res2", "y", "o_hi", "o_lo", "gn_partial"};
+  bool known = false;
+  for (const char* n : names) known = known || strcmp(n, what) == 0;
+  if (!known) return fail(FEMASR_ERR_ARG, std::string("set_conv_capture: unknown operand ") + what);
+  if (dst) net->captures[{ordinal, what}] = Capture{dst, bytes};
+  else net->captures.erase({ordinal, what});
+  return FEMASR_OK;
+}
+
+extern "C" const char* femasr_net_conv_trace_json(femasr_net* net) {
+  if (!net) return "[]";
+  static const char* pro[] = {"none", "gn", "ln", "gn_fast"};
+  static const char* res1[] = {"none", "sep", "alias"};
+  static const char* operand[] = {"staged", "planes", "im2col"};
+  auto b = [](bool v) { return v ? "true" : "false"; };
+  std::string js = "[";
+  for (size_t i = 0; i < net->trace.size(); ++i) {
+    const ConvRec& r = net->trace[i];
+    char buf[1024];
+    snprintf(buf, sizeof(buf),
+             "%s{\"ordinal\": %zu, \"w\": \"%s\", \"B\": %d, \"H\": %d, \"W\": %d, \"Cin\": %d, \"Cout\": %d, \"k\": %d, "
+             "\"stride\": %d, \"upsample\": %d, \"path\": \"%s\", \"prologue\": \"%s\", \"act\": %d, \"bias\": %s, "
+             "\"res1\": \"%s\", \"res2\": %s, \"out\": \"%s\", \"gn_partial\": %s, \"operand\": \"%s\", \"semantic\": %s, "
+             "\"sn\": %s, \"slice_kb\": %d, \"f8\": %s, \"precise_region\": %s}",
+             i ? ", " : "", i, r.w.c_str(), r.B, r.H, r.W, r.Cin, r.Cout, r.k, r.stride, r.upsample, r.tc ? "tc" : "simt",
+             pro[r.pro], r.act, b(r.bias), res1[r.res1], b(r.res2), r.split ? "split" : "f32", b(r.gn_partial),
+             operand[r.operand], b(r.semantic), b(r.sn), r.slice_kb, b(r.f8), b(r.precise_region));
+    js += buf;
+  }
+  net->trace_json = js + "]";
+  return net->trace_json.c_str();
 }
 
 extern "C" int femasr_net_last_launch_count(femasr_net* net) { return net ? net->last_launches : 0; }

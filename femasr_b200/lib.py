@@ -82,6 +82,8 @@ SIGNATURES = {
     "femasr_net_decode_indices": (_I, [_V, _V, _V, _I, _I, _I, _V, _Z, _V]),
     "femasr_net_decode_workspace_bytes": (_I, [_V, _I, _I, _I, C.POINTER(_Z)]),
     "femasr_net_set_tap": (_I, [_V, C.c_char_p, _V, _Z]),
+    "femasr_net_conv_trace_json": (C.c_char_p, [_V]),
+    "femasr_net_set_conv_capture": (_I, [_V, _I, C.c_char_p, _V, _Z]),
     "femasr_net_last_launch_count": (_I, [_V]),
     "femasr_net_set_profile": (_I, [_V, _I]),
     "femasr_net_profile_json": (C.c_char_p, [_V]),

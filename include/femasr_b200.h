@@ -119,6 +119,22 @@ int femasr_net_decode_workspace_bytes(femasr_net* net, int B, int h, int w, size
  * second / third codebook), vgg (relu4_4) and semantic (ReLU(conv_semantic(z_quant))), the last two only in a
  * forward that computes the semantic loss.  dst == NULL removes the tap. */
 int femasr_net_set_tap(femasr_net* net, const char* stage, float* dst, size_t capacity);
+/* Testing aid for every handle kind: the conv / linear layers (the implicit GEMM calls) of the handle's last run, sizing
+ * runs (femasr_net_workspace_bytes*, femasr_net_flops, the disc / LPIPS equivalents) included, as a JSON list in launch
+ * order.  Each record: ordinal, w (the weight's parameter name), B, H, W (the GEMM's input size; the output size for
+ * the im2col GEMMs), Cin, Cout, k, stride, upsample, path (tc | simt), prologue as staged (none | gn | gn_fast | ln),
+ * act (FEMASR_ACT_*), bias, res1 (none | sep | alias: the output buffer), res2, out (f32 | split), gn_partial, operand
+ * (staged: from fp32 x | planes: split planes a producer wrote | im2col: rows of a 3-channel first conv), semantic, sn,
+ * slice_kb, f8, precise_region.  Built on the host; valid until the next call. */
+const char* femasr_net_conv_trace_json(femasr_net* net);
+/* Testing aid for every handle kind: in the following real runs, copy operand `what` of the conv with trace ordinal
+ * `ordinal` into the device buffer dst of `bytes` bytes, stream-ordered like a tap.  what: x (fp32 input), a_hi, a_lo
+ * (fp16 planes a producer wrote), pa, pb (GroupNorm scale / shift [B,Cin], or LayerNorm mean / rstd [B*H*W] on
+ * gemm_path 0), res1, res2 (copied before the launch, so res1 is the residual even when it is the output buffer), y
+ * (fp32 output), o_hi, o_lo (split output planes), gn_partial (the output's GroupNorm partials).  Several captures may be
+ * registered at once; dst == NULL removes one.  A run fails with FEMASR_ERR_ARG when a buffer is too small, or when a
+ * registered ordinal / operand does not occur in it.  Launch counts, workspace bytes and FLOPs are unaffected. */
+int femasr_net_set_conv_capture(femasr_net* net, int ordinal, const char* what, void* dst, size_t bytes);
 /* Number of kernels the last femasr_net_forward launched (bench.py's gpu_launches). */
 int femasr_net_last_launch_count(femasr_net* net);
 /* Per-kernel timing for bench.py's roofline: while enabled, every launch of femasr_net_forward is

@@ -3,10 +3,12 @@
 
 One table of conv classes (CLASSES), one runner (run_case), one reference (reference).  A class is what Ctx::conv composes:
 kernel size, stride, fused upsample, prologue, activation, bias, residuals, output form, GroupNorm partials, operand form,
-numerics and channels.  CLASSES holds every class Ctx::forward, decode_loop, swin, resblock, up_block, quantise
-(before_quant), semantic_loss, vgg_stack, alex and disc emit on gemm_path 1 for the configurations of
-tests/test_engine_plan.py (CONFIGS and HEADS); the numerics column follows Ctx::numerics.  The quantiser's z . E^T is not a
-conv there: with the fused VQ (the default) it is femasr_vq_match_tc, which tests/test_vq_fused_gpu.py covers.
+numerics and channels.  CLASSES holds exactly the classes and channel pairs Ctx::conv launches on gemm_path 1 for the
+configurations of tests/test_engine_plan.py (CONFIGS and HEADS); tests/test_conv_trace.py checks this both ways against
+the engine's conv trace, and that every gemm_path 0 launch is a class check_simt runs.  The numerics column follows
+Ctx::numerics.  The quantiser's z . E^T is not a conv on gemm_path 1: with the fused VQ (the default) it is
+femasr_vq_match_tc, which tests/test_vq_fused_gpu.py covers.  tests/test_engine_convs_gpu.py holds every launch of the
+engine's networks to the bars of this file (tc_bar, SIMT_BAR).
 
 Every class runs at three spatial shapes chosen for the kernel's 128-pixel tiles (Wt x Ht, tc_tile_shape in tc_gemm.cu,
 mirrored by tile_shape below): an exact fit, a ragged multi-tile batch of 2 with odd sizes, and wide rows with Wt = 128.
@@ -71,6 +73,8 @@ CLASSES = [
     # swin: qkv and fc1 stage LayerNorm; proj and fc2 read planes (attention output, fc1's split output)
     Cls("swin_qkv", ((256, 768),), k=1, pro="ln"),
     Cls("swin_proj", ((256, 256),), k=1, operand="planes", res1="sep"),
+    # blocks 1-5 of a residual group: proj adds its residual into its own output buffer (the token tensor T)
+    Cls("swin_proj_alias", ((256, 256),), k=1, operand="planes", res1="alias"),
     Cls("swin_fc1", ((256, 1024),), k=1, pro="ln", act=GELU, out="split"),
     Cls("swin_fc2", ((1024, 256),), k=1, operand="planes", res1="alias", num="slice"),
     Cls("swin_conv", ((256, 256),), res1="alias", num="slice"),
@@ -130,8 +134,10 @@ ACCEPTED = [(Cls(f"act{act}_k{k}", A, k=k, stride=2 if k == 4 else 1, act=act), 
     (Cls("k5_stride2", A, k=5, stride=2), "refused"),
 ]
 SIMT_REFUSES = {"up_k1", "k4_stride1", "k5_stride2"}        # the rows femasr_igemm_simt refuses as well
-# femasr_igemm_simt alone: its k-step is 16 channels, and Cin % 16 is all its argument check asks
-SIMT_ONLY = [Cls("simt_cin48", ((48, 64),), res1="sep"), Cls("simt_cin80", ((80, 128),), k=1, act=GELU)]
+# femasr_igemm_simt alone: its k-step is 16 channels, and Cin % 16 is all its argument check asks; and the quantiser's
+# z . E^T on gemm_path 0 (a 1x1 without bias over the codebook)
+SIMT_ONLY = [Cls("simt_cin48", ((48, 64),), res1="sep"), Cls("simt_cin80", ((80, 128),), k=1, act=GELU),
+             Cls("simt_z_et", ((256, 1024), (128, 512)), k=1, bias=False)]
 
 
 # ------------------------------------------------------------------------------------------------ shapes
@@ -392,10 +398,32 @@ def check_simt(c, d, what):
     return e
 
 
+def check_gn_partials(part, y32, what):
+    """GroupNorm partials [B, rows, 32, 2] of the fp32 output y32 [B, Ho, Wo, Cout] (device tensors): summed over rows in
+    fp64 they are the per-(image, group) sum and sum of squares of y32, and femasr_gn_finalize_rows turns them into the
+    scale / shift a stats pass over y32 gives."""
+    lib = L.load()
+    B, Ho, Wo, cout = y32.shape
+    cpg = cout // 32
+    v = y32.double().view(B, -1, 32, cpg)
+    s, ss = v.sum((1, 3)), (v * v).sum((1, 3))
+    ps = part.double().sum(1)
+    count = v.shape[1] * cpg
+    assert ((ps[..., 1] - ss).abs() <= 1e-6 * ss).all(), f"{what}: sum of squares partials"
+    assert ((ps[..., 0] - s).abs() <= 1e-6 * count).all(), f"{what}: sum partials"
+    g = torch.Generator().manual_seed(7)
+    gamma, beta = (1 + 0.2 * rnd(g, cout)).to(y32.device), (0.2 * rnd(g, cout)).to(y32.device)
+    sc, sh = torch.empty(B, cout, device=y32.device), torch.empty(B, cout, device=y32.device)
+    L.check(lib.femasr_gn_finalize_rows(G.p(part), G.p(gamma), G.p(beta), G.p(sc), G.p(sh), B, part.shape[1], Ho * Wo,
+                                        cout, 1e-6, G.S()))
+    sc2, sh2 = G.gn_tables(y32.contiguous(), gamma, beta)
+    assert (sc - sc2).abs().max().item() <= 2e-6 * sc2.abs().max().item(), f"{what}: finalize_rows scale"
+    assert (sh - sh2).abs().max().item() <= 2e-6 * max(1.0, sh2.abs().max().item()), f"{what}: finalize_rows shift"
+
+
 def check_tc(c, d, what):
     """femasr_tc_igemm: accuracy, canaries, split-output bits, GroupNorm partials, in-place equality."""
-    lib = L.load()
-    want, B, cout = d["want"], d["B"], d["cout"]
+    want, B = d["want"], d["B"]
     op = tc_operand(c, d)
     out, part, bufs = tc_call(c, d, op)
     for k, buf in bufs.items():
@@ -415,22 +443,7 @@ def check_tc(c, d, what):
     bar = tc_bar(c)
     assert e <= bar, f"{what}: rel err {e:.3e} > {bar:.1e}; {describe(got, want, c, B, d['H'], d['W'])}"
     if c.gn:
-        # summed over rows in fp64, the partials are the per-(image, group) sum and sum of squares of the stored output
-        cpg = cout // 32
-        v = y32.double().view(B, -1, 32, cpg)
-        s, ss = v.sum((1, 3)), (v * v).sum((1, 3))
-        ps = part.double().sum(1)
-        count = v.shape[1] * cpg
-        assert ((ps[..., 1] - ss).abs() <= 1e-6 * ss).all(), f"{what}: sum of squares partials"
-        assert ((ps[..., 0] - s).abs() <= 1e-6 * count).all(), f"{what}: sum partials"
-        g = torch.Generator().manual_seed(7)
-        gamma, beta = (1 + 0.2 * rnd(g, cout)).to(y32.device), (0.2 * rnd(g, cout)).to(y32.device)
-        sc, sh = torch.empty(B, cout, device=y32.device), torch.empty(B, cout, device=y32.device)
-        L.check(lib.femasr_gn_finalize_rows(G.p(part), G.p(gamma), G.p(beta), G.p(sc), G.p(sh), B, part.shape[1],
-                                            d["Ho"] * d["Wo"], cout, 1e-6, G.S()))
-        sc2, sh2 = G.gn_tables(y32.contiguous(), gamma, beta)
-        assert (sc - sc2).abs().max().item() <= 2e-6 * sc2.abs().max().item(), f"{what}: finalize_rows scale"
-        assert (sh - sh2).abs().max().item() <= 2e-6 * max(1.0, sh2.abs().max().item()), f"{what}: finalize_rows shift"
+        check_gn_partials(part, y32, what)
     if c.res1 == "alias":
         out2, part2, bufs2 = tc_call(c, d, op, alias=True, split=False)
         assert_canaries(bufs2["y"], f"{what} y in place")
