@@ -100,13 +100,6 @@ __device__ __forceinline__ float2 lds_f2(uint32_t a) {
 __device__ __forceinline__ void sts_f2(uint32_t a, float2 v) { asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v.x), "f"(v.y)); }
 __device__ __forceinline__ void sts_u32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v)); }
 
-// Programmatic dependent launch: a kernel launched with the programmatic-serialisation attribute may start (its CTAs
-// become resident as the predecessor's retire, it runs its prologue) before the predecessor has finished;
-// griddepcontrol.wait blocks until the predecessor grid has completed and its memory is visible.  Both are no-ops in a
-// plain launch.
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
 // One lane of a converged warp (elect.sync): the TMA producer role is entered through this instead of `lane == 0` so
 // that ptxas knows a single lane issues the loads (no per-load serialisation loop).
 __device__ __forceinline__ bool elect_one() {
@@ -685,7 +678,6 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
   float* red = reinterpret_cast<float*>(smem_raw + (r.bar_base + 256u - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  pdl_launch_dependents();        // the next kernel of the stream may begin its own prologue as our CTAs retire
   if (threadIdx.x == 0) {
     // a stage (column box) is released by every warp that reads it: all consumer warps, or (PP) one warpgroup's
     constexpr int READERS = PP ? TC_CONSUMER_WARPS / 2 : TC_CONSUMER_WARPS;
@@ -695,7 +687,6 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  pdl_wait();                     // barriers initialised: from here on the predecessor's output is read
 
   if (PP ? warp >= TC_CONSUMER_WARPS : warp == TC_CONSUMER_WARPS) {
     if constexpr (PP) {
@@ -963,8 +954,6 @@ template <int MODE>
 __global__ void __launch_bounds__(256) tc_prepare_flat_kernel(const float4* __restrict__ x, uint2* __restrict__ hi,
                                                               uint2* __restrict__ lo, const float* __restrict__ sc,
                                                               const float* __restrict__ sh, int C, int per_image4) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int b = blockIdx.y;
   const long base = (long)b * per_image4;
   const int i0 = blockIdx.x * (256 * PREP_U) + threadIdx.x;
@@ -1083,8 +1072,6 @@ __global__ void __launch_bounds__(256) tc_prepare_flat_f8_kernel(const float4* _
 __global__ void __launch_bounds__(256) tc_prepare_ln_kernel(const float* __restrict__ x, __half* __restrict__ hi,
                                                             __half* __restrict__ lo, const float* __restrict__ gamma,
                                                             const float* __restrict__ beta, long M, float eps) {
-  pdl_launch_dependents();
-  pdl_wait();
   // two rows per warp, all four 512-byte requests of the warp in flight before the first reduction
   constexpr int LN_ROWS = 2;
   const long row0 = ((long)blockIdx.x * 8 + (threadIdx.x >> 5)) * LN_ROWS;
@@ -1243,28 +1230,6 @@ static int make_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t*
   return FEMASR_OK;
 }
 
-// Launch with the programmatic-stream-serialisation attribute when FEMASR_PDL=1.  Only kernels that execute
-// griddepcontrol.wait before their first dependent global access are launched this way.  Off by default: the persistent
-// GEMM CTAs take a whole SM's shared memory and cannot become resident before the predecessor's CTAs retire anyway.
-static bool pdl_enabled() {
-  static const int env = [] { const char* e = getenv("FEMASR_PDL"); return e ? atoi(e) : 0; }();
-  return env != 0;
-}
-template <class... KArgs, class... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  int n = 0;
-  if (pdl_enabled()) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  cfg.attrs = attr; cfg.numAttrs = n;
-  return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
-}
-
 // The four operand maps of a launch: A = the NHWC fp16 planes [B][H][W][C] in 4-D boxes of 64 ch x box_w x box_h x 1,
 // traversed with the spatial stride `stride`; B = the K-major weight planes [rows][K] in 2-D boxes of 64 x BN.
 // TMAE launches add the output and residual maps (tc_tma_epi_maps); the others pass them unset.
@@ -1312,8 +1277,8 @@ static int launch_tc_v(const TcMaps& m, const TcP& p, cudaStream_t st) {
   }
   const int items = VQ ? p.num_tiles / p.n_tiles : p.num_tiles;     // VQ: one CTA walks all code tiles of an m-tile
   const int grid = items < sm_count() ? items : sm_count();
-  FEMASR_CUDA(launch_pdl(tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP, TMAE>, dim3(grid), dim3(PP ? TC_PP_THREADS : TC_THREADS),
-                         Cfg::SMEM_BYTES, st, m.a_hi, m.a_lo, m.b_hi, m.b_lo, p, m.o0, m.o1, m.res));
+  tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP, TMAE><<<grid, PP ? TC_PP_THREADS : TC_THREADS, Cfg::SMEM_BYTES, st>>>(
+      m.a_hi, m.a_lo, m.b_hi, m.b_lo, p, m.o0, m.o1, m.res);
   return launch_status(VQ ? "tc_igemm_kernel(vq)" : "tc_igemm_kernel");
 }
 
@@ -1327,8 +1292,11 @@ static int launch_tc(const TcMaps& m, const TcP& p, cudaStream_t st) {
 }
 template <int BN, bool PP>
 static int launch_tc(const TcMaps& m, const TcP& p, bool cols, cudaStream_t st) {
-  if (cols) return launch_tc<BN, PP, true, true, 0>(m, p, st);
-  if (p.f8) return launch_tc<BN, PP, false, true, 0>(m, p, st);
+  if (p.f8) {
+    // F8 is never K-sliced, so BN-64 F8 always runs ping-pong: the cooperative BN-64 schedule has no F8 kernels
+    if constexpr (BN == 64 && !PP) return fail(FEMASR_ERR_ARG, "tc_igemm: no cooperative BN-64 F8 kernel");
+    else return cols ? launch_tc<BN, PP, true, true, 0>(m, p, st) : launch_tc<BN, PP, false, true, 0>(m, p, st);
+  }
   if (p.taps == 25) return launch_tc<BN, PP, false, false, 2>(m, p, st);
   if (p.taps == 16 || p.act == FEMASR_ACT_LRELU) return launch_tc<BN, PP, false, false, 1>(m, p, st);
   return launch_tc<BN, PP, false, false, 0>(m, p, st);
@@ -1354,36 +1322,32 @@ static void tc_tile_shape(int H, int W, int* Wt, int* Ht) {
 // schedules of other GPU generations and do not change the tiling here.
 // The stride-1 3x3 convs in F8 mode over the whole K range run the column schedule (8 x 16 tiles, TcCfg) wherever it
 // needs no more tiles than tc_tile_shape's choice: every map behind the VQ, whose sides are multiples of 16.  The tile
-// count, and with it the GroupNorm partial-row count, is then the same for both schedules.  FEMASR_TC_COLUMNS=0 keeps
-// the tap-order schedule (for A/B timing).
+// count, and with it the GroupNorm partial-row count, is then the same for both schedules.
 // The ping-pong schedule (tc_igemm_kernel's PP) runs the BN-64 launches that are not K-sliced (`sliced`: the launch's
 // effective slicing); a warpgroup holds a whole 128 x 64 tile, F8 accumulator included.  BN 128 keeps the cooperative
 // schedule: with F8 or K slicing its two accumulators do not fit in one warpgroup, and without them (the linears)
 // ping-pong measured slower on H100 - their short k-loops cannot hide an epilogue that one warpgroup runs alone.  It
-// changes neither the tiling nor any sum.  FEMASR_TC_PINGPONG=0 keeps the cooperative schedule (for A/B timing).
+// changes neither the tiling nor any sum.
 // The TMA epilogue (tc_igemm_kernel's TMAE) runs the cooperative BN-128 1x1 launches without F8, GroupNorm partials,
 // res2 or LeakyReLU, and without a residual beside a split output (the Swin linears, the 1x1s before the VQ, the im2col
 // first-conv GEMM at Cout 128 / 256, conv_semantic): their short k-loops left the tensor cores idle while the register
-// epilogue waited on global memory.  FEMASR_TC_TMA_EPILOGUE=0 keeps the register epilogue (for A/B timing).
+// epilogue waited on global memory.
 struct TilePlan { int Wt, Ht, wt_shift, tiles_x, tiles_y, BN; bool cols, pingpong, tma_epilogue; };
 static TilePlan plan_tiles(const femasr_tc_args* a, int H, int W, bool sliced = false) {
-  static const int cols_env = [] { const char* e = getenv("FEMASR_TC_COLUMNS"); return e ? atoi(e) : 1; }();
-  static const int pp_env = [] { const char* e = getenv("FEMASR_TC_PINGPONG"); return e ? atoi(e) : 1; }();
-  static const int tma_env = [] { const char* e = getenv("FEMASR_TC_TMA_EPILOGUE"); return e ? atoi(e) : 1; }();
   TilePlan t;
   t.BN = a->Cout % 128 == 0 ? 128 : 64;
   tc_tile_shape(H, W, &t.Wt, &t.Ht);   // the widest power-of-two Wt <= 128 that wastes the fewest padded pixels
   t.tiles_x = (int)cdiv(W, t.Wt); t.tiles_y = (int)cdiv(H, t.Ht);
   const long nkb = 9l * (a->Cin / 64);
-  t.cols = cols_env && a->f8 && a->ksize == 3 && a->stride != 2 && !a->upsample && a->kb_begin == 0 &&
+  t.cols = a->f8 && a->ksize == 3 && a->stride != 2 && !a->upsample && a->kb_begin == 0 &&
            (a->kb_count == 0 || a->kb_count == nkb) && cdiv(W, COL_WT) * cdiv(H, COL_HT) == (long)t.tiles_x * t.tiles_y;
   if (t.cols) { t.Wt = COL_WT; t.Ht = COL_HT; t.tiles_x = (int)cdiv(W, COL_WT); t.tiles_y = (int)cdiv(H, COL_HT); }
   t.wt_shift = 0; while ((1 << t.wt_shift) < t.Wt) ++t.wt_shift;
-  t.pingpong = pp_env && !sliced && t.BN == 64;
+  t.pingpong = !sliced && t.BN == 64;
   // 16-byte aligned outputs and residual: the TMA maps' global addresses
   auto al16 = [](const void* q) { return ((uintptr_t)q & 15u) == 0; };
   const bool split = a->out_hi != nullptr;
-  t.tma_epilogue = tma_env && t.BN == 128 && !t.pingpong && !t.cols && a->ksize == 1 && !a->f8 && !a->gn_partial &&
+  t.tma_epilogue = t.BN == 128 && !t.pingpong && !t.cols && a->ksize == 1 && !a->f8 && !a->gn_partial &&
                    !a->res2 && a->act != FEMASR_ACT_LRELU && !(split && a->res1) &&
                    (split ? al16(a->out_hi) && al16(a->out_lo) : al16(a->y)) && (!a->res1 || al16(a->res1));
   return t;
@@ -1486,7 +1450,7 @@ extern "C" int femasr_tc_prepare(const float* x, void* a_hi, void* a_lo, int mod
   if (mode == FEMASR_PRO_LN) {
     FEMASR_CHECK_ARG(C == 256 && gamma && beta && !upsample, "tc_prepare: LN mode needs C=256, gamma/beta, no upsample");
     const long M = (long)B * H * W;
-    FEMASR_CUDA(launch_pdl(tc_prepare_ln_kernel, dim3((unsigned)cdiv(M, 16)), dim3(256), 0, st, x, hi, lo, gamma, beta, M, eps));
+    tc_prepare_ln_kernel<<<(unsigned)cdiv(M, 16), 256, 0, st>>>(x, hi, lo, gamma, beta, M, eps);
     return launch_status("tc_prepare_ln_kernel");
   }
   if (mode == FEMASR_PRO_MAXPOOL2) {
@@ -1507,20 +1471,21 @@ extern "C" int femasr_tc_prepare(const float* x, void* a_hi, void* a_lo, int mod
     tc_prepare_bilinear_kernel<<<(unsigned)cdiv(total8, 256), 256, 0, st>>>(x, hi, lo, H, W, C, total8);
     return launch_status("tc_prepare_bilinear_kernel");
   }
-  static const int flat_env = [] { const char* e = getenv("FEMASR_PREP_FLAT"); return e ? atoi(e) : 1; }();
-  if (!upsample && flat_env && (long)H * W * (C / 4) < (1l << 30) && B <= 65535 &&
+  if (!upsample && (long)H * W * (C / 4) < (1l << 30) && B <= 65535 &&
       (mode == FEMASR_PRO_GN_SILU || mode == FEMASR_PRO_GN_SILU_FAST || mode == FEMASR_PRO_NONE)) {
     const int per4 = H * W * (C / 4);
     const dim3 grid((unsigned)cdiv(per4, 256 * PREP_U), (unsigned)B);
     const float4* x4 = reinterpret_cast<const float4*>(x);
+    uint2* hi4 = reinterpret_cast<uint2*>(hi);
+    uint2* lo4 = reinterpret_cast<uint2*>(lo);
     if (mode == FEMASR_PRO_GN_SILU) {
       FEMASR_CHECK_ARG(pro_a && pro_b, "tc_prepare: GN mode needs the scale/shift tables");
-      FEMASR_CUDA(launch_pdl(tc_prepare_flat_kernel<FEMASR_PRO_GN_SILU>, grid, dim3(256), 0, st, x4, reinterpret_cast<uint2*>(hi), reinterpret_cast<uint2*>(lo), pro_a, pro_b, C, per4));
+      tc_prepare_flat_kernel<FEMASR_PRO_GN_SILU><<<grid, 256, 0, st>>>(x4, hi4, lo4, pro_a, pro_b, C, per4);
     } else if (mode == FEMASR_PRO_GN_SILU_FAST) {
       FEMASR_CHECK_ARG(pro_a && pro_b, "tc_prepare: GN mode needs the scale/shift tables");
-      FEMASR_CUDA(launch_pdl(tc_prepare_flat_kernel<FEMASR_PRO_GN_SILU_FAST>, grid, dim3(256), 0, st, x4, reinterpret_cast<uint2*>(hi), reinterpret_cast<uint2*>(lo), pro_a, pro_b, C, per4));
+      tc_prepare_flat_kernel<FEMASR_PRO_GN_SILU_FAST><<<grid, 256, 0, st>>>(x4, hi4, lo4, pro_a, pro_b, C, per4);
     } else {
-      FEMASR_CUDA(launch_pdl(tc_prepare_flat_kernel<FEMASR_PRO_NONE>, grid, dim3(256), 0, st, x4, reinterpret_cast<uint2*>(hi), reinterpret_cast<uint2*>(lo), (const float*)nullptr, (const float*)nullptr, C, per4));
+      tc_prepare_flat_kernel<FEMASR_PRO_NONE><<<grid, 256, 0, st>>>(x4, hi4, lo4, nullptr, nullptr, C, per4);
     }
     return launch_status("tc_prepare_flat_kernel");
   }

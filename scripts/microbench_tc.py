@@ -1,35 +1,7 @@
 """Per-shape timing of the tensor-core implicit GEMM through the C ABI (CUDA events, L2 flushed between reps).
 Usage (GPU box): python scripts/microbench_tc.py > gpurun_out/microbench.txt"""
 import os
-import subprocess
 import sys
-
-# MB_COLUMNS=ab: the F8 3x3 cases twice, on the column schedule (FEMASR_TC_COLUMNS=1) and on the tap-order one (=0)
-if os.environ.get('MB_COLUMNS') == 'ab':
-    for v in ('1', '0'):
-        print(f"# FEMASR_TC_COLUMNS={v}", flush=True)
-        env = dict(os.environ, MB_COLUMNS='', MB_F8='1', MB_ONLY=os.environ.get('MB_ONLY') or 'conv', FEMASR_TC_COLUMNS=v)
-        subprocess.run([sys.executable, os.path.abspath(__file__)], env=env, check=True)
-    sys.exit(0)
-# MB_PINGPONG=ab: the cases the ping-pong schedule runs (BN 64; BN 128 with no F8 / K-slice accumulator) on it
-# (FEMASR_TC_PINGPONG=1) and on the cooperative one (=0), the 3x3 convs in F8 mode with GroupNorm partials as in the
-# network; the K-sliced fc2 runs the cooperative schedule both times (a control)
-if os.environ.get('MB_PINGPONG') == 'ab':
-    for v in ('1', '0'):
-        print(f"# FEMASR_TC_PINGPONG={v}", flush=True)
-        env = dict(os.environ, MB_PINGPONG='', MB_F8='1', MB_GN='1', FEMASR_TC_PINGPONG=v,
-                   MB_ONLY=os.environ.get('MB_ONLY') or 'qkv|proj|fc1|fc2|64->64 @512|up 128->64')
-        subprocess.run([sys.executable, os.path.abspath(__file__)], env=env, check=True)
-    sys.exit(0)
-
-# MB_TMAEPI=ab: the linears the TMA epilogue runs (the Swin linears at the engine's geometry) with it
-# (FEMASR_TC_TMA_EPILOGUE=1) and with the register epilogue (=0)
-if os.environ.get('MB_TMAEPI') == 'ab':
-    for v in ('1', '0'):
-        print(f"# FEMASR_TC_TMA_EPILOGUE={v}", flush=True)
-        env = dict(os.environ, MB_TMAEPI='', FEMASR_TC_TMA_EPILOGUE=v, MB_ONLY=os.environ.get('MB_ONLY') or 'qkv|proj|fc1|fc2')
-        subprocess.run([sys.executable, os.path.abspath(__file__)], env=env, check=True)
-    sys.exit(0)
 
 import torch
 
@@ -53,8 +25,6 @@ def timeit(fn, reps=5):
     return ts[len(ts) // 2]
 
 
-PAIR = int(os.environ.get('MB_PAIR', '-1'))
-STRIP = int(os.environ.get('MB_STRIP', '-1'))
 ONLY = os.environ.get('MB_ONLY', '')        # substring filter on the case name ('|' separates alternatives)
 F8 = int(os.environ.get('MB_F8', '0'))      # 1: the 3x3 convs in the F8 cross-term mode (layers behind the VQ)
 GN = int(os.environ.get('MB_GN', '0'))      # 1: the 3x3 convs also emit GroupNorm partial sums (what most of them do in the network)
@@ -80,8 +50,8 @@ def conv_case(name, B, H, W, Cin, Cout, ksize=3, up=0, res=False, act=0, split=F
         y = r
     gn = None
     if GN and ksize == 3 and not split:
-        gn = torch.empty(B * G.tc_gn_rows(B, H, W, Cin, Cout, upsample=up, slice_kb=slice_kb, pair=PAIR, strip=STRIP) * 64, device=dev)
-    fn = lambda: G.tc_igemm(hi, lo, blob, b, Cout, ksize, act=act, res1=r, y=y, upsample=up, split_out=split, pair=PAIR, strip=STRIP, slice_kb=slice_kb, f8=f8, gn_partial=gn)
+        gn = torch.empty(B * G.tc_gn_rows(B, H, W, Cin, Cout, upsample=up, slice_kb=slice_kb) * 64, device=dev)
+    fn = lambda: G.tc_igemm(hi, lo, blob, b, Cout, ksize, act=act, res1=r, y=y, upsample=up, split_out=split, slice_kb=slice_kb, f8=f8, gn_partial=gn)
     ms = timeit(fn)
     flops = 2.0 * B * H * u * W * u * Cout * Cin * ksize * ksize
     execd = (2 if f8 else 3) * 2.0 * B * H * W * Cout * Cin * (4 * 4 if up else ksize * ksize)

@@ -1,17 +1,15 @@
-"""The TMA epilogue of the tensor-core implicit GEMM (FEMASR_TC_TMA_EPILOGUE, tc_igemm_kernel's TMAE): the cooperative
-BN-128 linears write each finished tile into shared memory and store it by TMA, with the residual tile loaded by TMA.
-Only how the bytes travel changes, not the rule per element, so every output must equal the register epilogue's byte for
-byte.  The environment variable is read once per process: each value runs in a subprocess of its own.
+"""The TMA epilogue of the tensor-core implicit GEMM (tc_igemm_kernel's TMAE): the cooperative BN-128 linears write each
+finished tile into shared memory and store it by TMA, with the residual tile loaded by TMA.  Only how the bytes travel
+changes, not the rule per element, so every output must equal the register epilogue's byte for byte.  plan_tiles takes
+the TMA epilogue only when the outputs and the residual are 16-byte aligned (the tensor maps' global addresses), so each
+case runs twice: on aligned buffers (TMA epilogue) and with the outputs and a separate residual placed 8 bytes past a
+16-byte boundary (register epilogue; 8 rather than 4 because that epilogue stores float2).
 
 Covered: qkv (fp32 out), proj with a separate and with an aliased residual (y == res1), fc1 (GELU, split fp16 out), fc2
 (K-sliced, aliased residual) and a ReLU 1x1, on 64x64, 24x40 and 7x9 maps at batch 1-3 and on a 4000-token row, so
 that tiles cross image boundaries and the last tile is ragged.  Every output lies inside a sentinel-filled guard
-allocation whose bytes outside the output must survive.  One small engine forward must also be identical under both
-values.  The outputs are checked against fp64 with tests/test_gemm_matrix_gpu.py's bars."""
-import os
-import subprocess
-import sys
-
+allocation whose bytes outside the output must survive.  The outputs are checked against fp64 with
+tests/test_gemm_matrix_gpu.py's bars."""
 import pytest
 import torch
 
@@ -22,6 +20,7 @@ pytestmark = pytest.mark.gpu
 RELU, GELU = 2, 1
 GUARD = 4096                        # guard elements on each side of an output (16-byte multiples: TMA alignment)
 SENT32, SENT16 = 0x7FC0DEAD, 0x7E5A  # NaN patterns no kernel writes
+EPILOGUES = {"tma": 0, "register": 8}  # bytes the outputs and a separate residual sit past a 16-byte boundary
 
 
 def cases():
@@ -52,15 +51,20 @@ def data(name, c):
     return x, w, b, r
 
 
-def guarded(n, dtype, sentinel, cuda):
+def start(dtype, shift):
+    """index of the output in its guard allocation: GUARD elements plus `shift` bytes"""
+    return GUARD + shift // dtype.itemsize
+
+
+def guarded(n, dtype, sentinel, shift, cuda):
     """(whole guard allocation, the n-element output inside it)"""
     idt = torch.int32 if dtype == torch.float32 else torch.int16
     buf = torch.full((n + 2 * GUARD,), sentinel, dtype=idt, device=cuda).view(dtype)
-    return buf, buf[GUARD:GUARD + n]
+    return buf, buf[start(dtype, shift):start(dtype, shift) + n]
 
 
-def run(name, c, cuda):
-    """The launch under the current knob value: {outputs, guard_ok} on the CPU."""
+def run(name, c, shift, cuda):
+    """The launch with its outputs `shift` bytes past a 16-byte boundary: {outputs, guard_ok} on the CPU."""
     B, H, W, Cin, Cout, act, res, split, slice_kb = c
     x, w, b, r = data(name, c)
     hi, lo = G.tc_prepare(G.nhwc(x).to(cuda))
@@ -70,17 +74,17 @@ def run(name, c, cuda):
     bufs = {}
     r1 = y = planes = None
     if split:
-        bufs["hi"], oh = guarded(n, torch.float16, SENT16, cuda)
-        bufs["lo"], ol = guarded(n, torch.float16, SENT16, cuda)
+        bufs["hi"], oh = guarded(n, torch.float16, SENT16, shift, cuda)
+        bufs["lo"], ol = guarded(n, torch.float16, SENT16, shift, cuda)
         planes = (oh.view(shape), ol.view(shape))
     else:
-        bufs["y"], yv = guarded(n, torch.float32, SENT32, cuda)
+        bufs["y"], yv = guarded(n, torch.float32, SENT32, shift, cuda)
         y = yv.view(shape)
     if res == "alias":
         y.copy_(r.to(cuda))
         r1 = y
     elif res == "sep":
-        bufs["r"], rv = guarded(n, torch.float32, SENT32, cuda)
+        bufs["r"], rv = guarded(n, torch.float32, SENT32, shift, cuda)
         r1 = rv.view(shape)
         r1.copy_(r.to(cuda))
     G.tc_igemm(hi, lo, blob, b.to(cuda), Cout, 1, act=act, res1=r1, y=y, out_planes=planes, slice_kb=slice_kb)
@@ -88,49 +92,19 @@ def run(name, c, cuda):
     out = {"hi": planes[0].cpu(), "lo": planes[1].cpu()} if split else {"y": y.cpu()}
     guard_ok = {}
     for k, buf in bufs.items():
+        off = start(buf.dtype, shift)
         ints = buf.view(torch.int32 if buf.dtype == torch.float32 else torch.int16)
         s = SENT32 if buf.dtype == torch.float32 else SENT16
-        guard_ok[k] = bool((ints[:GUARD] == s).all() and (ints[GUARD + n:] == s).all())
+        guard_ok[k] = bool((ints[:off] == s).all() and (ints[off + n:] == s).all())
     if res == "sep":
         guard_ok["r_unchanged"] = torch.equal(r1.cpu(), r)
     return {"out": out, "guard_ok": guard_ok}
 
 
-def engine_forward(cuda):
-    """SR output, indices and loss of one small FeMaSRNet forward on the engine (as smoke())."""
-    from basicsr.archs import build_network
-    from femasr_b200.spec import random_state_dict
-    sd = random_state_dict(4, 256, seed=5, init="perturbed")
-    net = build_network(dict(type="FeMaSRNet", codebook_params=[[32, 1024, 256]], LQ_stage=True, scale_factor=4))
-    net.load_state_dict(sd, strict=True)
-    net = net.to(cuda).eval()
-    x = torch.rand(2, 3, 32, 48, generator=torch.Generator().manual_seed(6))
-    with torch.no_grad():
-        out, loss, _sem, idx = net(x.to(cuda))
-    torch.cuda.synchronize()
-    return {"out": out.cpu(), "loss": torch.as_tensor(loss).cpu(), "idx": idx[0].cpu()}
-
-
-def dump(path):
-    cuda = torch.device("cuda", 0)
-    res = {name: run(name, c, cuda) for name, c in cases().items()}
-    res["engine"] = engine_forward(cuda)
-    torch.save(res, path)
-
-
 @pytest.fixture(scope="module")
-def knob(cuda, tmp_path_factory):
-    """{knob value: results} from one subprocess per FEMASR_TC_TMA_EPILOGUE value."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = {}
-    for v in ("1", "0"):
-        path = str(tmp_path_factory.mktemp("tmae") / f"tmae{v}.pt")
-        env = dict(os.environ, FEMASR_TC_TMA_EPILOGUE=v, PYTHONPATH=os.pathsep.join([root, os.environ.get("PYTHONPATH", "")]))
-        r = subprocess.run([sys.executable, "-s", os.path.abspath(__file__), path], env=env, cwd=root,
-                           capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, r.stdout + r.stderr
-        out[v] = torch.load(path)
-    return out
+def runs(cuda):
+    """{name: {epilogue: results}}"""
+    return {name: {e: run(name, c, shift, cuda) for e, shift in EPILOGUES.items()} for name, c in cases().items()}
 
 
 def same_bytes(a, b):
@@ -146,25 +120,25 @@ NAMES = list(cases())
 
 
 @pytest.mark.parametrize("name", NAMES)
-def test_tc_tma_epilogue_equals_register_epilogue(knob, name):
-    tma, reg = knob["1"][name]["out"], knob["0"][name]["out"]
+def test_tc_tma_epilogue_equals_register_epilogue(runs, name):
+    tma, reg = runs[name]["tma"]["out"], runs[name]["register"]["out"]
     assert tma.keys() == reg.keys()
     for key in tma:
         assert same_bytes(tma[key], reg[key]), f"{name} {key}: {int((tma[key] != reg[key]).sum())} elements differ"
 
 
-@pytest.mark.parametrize("v", ["1", "0"])
+@pytest.mark.parametrize("epilogue", list(EPILOGUES))
 @pytest.mark.parametrize("name", NAMES)
-def test_tc_tma_epilogue_writes_only_the_output(knob, name, v):
-    bad = [k for k, ok in knob[v][name]["guard_ok"].items() if not ok]
+def test_tc_tma_epilogue_writes_only_the_output(runs, name, epilogue):
+    bad = [k for k, ok in runs[name][epilogue]["guard_ok"].items() if not ok]
     assert not bad, f"{name}: bytes outside the output changed in {bad}"
 
 
 @pytest.mark.parametrize("name", NAMES)
-def test_tc_tma_epilogue_against_fp64(knob, name):
+def test_tc_tma_epilogue_against_fp64(runs, name):
     c = cases()[name]
     B, H, W, Cin, Cout, act, res, split, slice_kb = c
-    got = knob["1"][name]["out"]
+    got = runs[name]["tma"]["out"]
     y = got["y"] if "y" in got else got["hi"].float() + got["lo"].float()
     x, w, b, r = data(name, c)
     want = torch.einsum("bchw,oc->bhwo", x.double(), w[:, :, 0, 0].double()) + b.double()
@@ -177,13 +151,3 @@ def test_tc_tma_epilogue_against_fp64(knob, name):
     e = ((y.double() - want).abs().max() / want.abs().max()).item()
     print(f"{name}: rel err {e:.2e}")
     assert e <= 2e-5 + (1e-5 if act == GELU else 0.0)      # test_gemm_matrix_gpu.tc_bar: one pass, GELU
-
-
-def test_tc_tma_epilogue_engine_forward_identical(knob):
-    a, b = knob["1"]["engine"], knob["0"]["engine"]
-    for key in a:
-        assert same_bytes(a[key], b[key]), f"engine forward {key} differs between the epilogues"
-
-
-if __name__ == "__main__":
-    dump(sys.argv[1])
