@@ -158,6 +158,11 @@ SIGNATURES = {
     "femasr_metric_scratch_bytes": (_Z, [_I, _I, _I, _I, _I]),
     "femasr_psnr": (_I, [_V, _V, _I, _I, _I, _I, _I, _V, _V, _V]),
     "femasr_ssim": (_I, [_V, _V, _I, _I, _I, _I, _I, _V, _V, _V]),
+    "femasr_degrade_mirror_conv": (_I, [_V, _V, _I, _I, _V, _I, _I, _I, _I, _V]),
+    "femasr_degrade_resize_pass": (_I, [_V, _V, _I, _I, _I, _I, _V, _V, _I, _I, _V]),
+    "femasr_degrade_noise_add": (_I, [_V, _V, _I, _I, _I, _V, _V]),
+    "femasr_degrade_jpeg_workspace_bytes": (_Z, [_I, _I]),
+    "femasr_degrade_jpeg": (_I, [_V, _V, _I, _I, _V, _V, _V]),
 }
 
 _lib = None

@@ -519,6 +519,41 @@ int femasr_psnr(const float* x, const float* y, int B, int H, int W, int crop, i
 int femasr_ssim(const float* x, const float* y, int B, int H, int W, int crop, int mode, float* out, void* scratch,
                 void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * BSRGAN degradation steps (degradation_bsrgan of the reference's basicsr/data/bsrgan_util.py), the synthesis of
+ * low-quality training inputs from HQ crops.  Images are [H, W, 3] fp32 HWC RGB device arrays; y must not alias x.
+ * The random draws, kernel taps and resize tables are made on the host (femasr_b200/degrade.py).  Every call refuses
+ * with FEMASR_ERR_ARG, giving the reason, a null pointer, H or W below 1, or an image above 2^28 pixels.
+ *
+ * femasr_degrade_mirror_conv: ndimage.convolve(x, k[..., None], mode='mirror') (the reflection about the edge samples,
+ *   folded as often as the radius needs), keeping output pixels [0::stride, 0::stride] only, so y is
+ *   [ceil(H/stride), ceil(W/stride), 3].  taps: the kh x kw kernel k, row-major fp64, on the host; kh, kw odd in
+ *   [1, 25]; stride in [1, 4].  Each output sums its products in fp64 (row-major over the flipped kernel, products and
+ *   sums rounded separately) and is rounded to fp32 once; clip 1 then clamps it to [0, 1].
+ * femasr_degrade_resize_pass: one separable pass of a resize along axis 0 (rows: y [out_n, W, 3]) or 1 (columns:
+ *   y [H, out_n, 3]).  idx [out_n][K] int32 and w [out_n][K] fp32 device tables: y[o] = sum_k w[o][k] x[idx[o][k]],
+ *   accumulated in fp32 in tap order, starting from the first product, without contraction (a zero weight pads a
+ *   shorter row exactly).  Indices must lie in [0, n) of that axis.  K in [1, 64]; clip 1 clamps to [0, 1].
+ * femasr_degrade_noise_add: y = clip(x + noise, 0, 1) in fp32: noise [H, W, noise_ch], noise_ch 3, or 1 broadcast over
+ *   the channels.
+ * femasr_degrade_jpeg: add_JPEG_noise: single2uint (round half to even of clip(x, 0, 1) * 255), then what
+ *   cv2.imencode('.jpg') / cv2.imdecode over libjpeg-turbo return: baseline 4:2:0 quantised by qtables (host, [2][64]
+ *   int in natural order, luma then chroma, entries in [1, 255]: the standard tables scaled by the quality, as
+ *   femasr_b200.degrade.jpeg_quant_tables builds them), islow FDCT and IDCT, h2v2 fancy upsampling (plain replication when ceil(W/2) <= 2),
+ *   fixed-point colour conversions, replicated edges; then uint2single (k / 255 rounded to fp32).  Exact: integer
+ *   arithmetic throughout.  workspace: femasr_degrade_jpeg_workspace_bytes(H, W) device bytes.
+ * ---------------------------------------------------------------------------------------------- */
+enum { FEMASR_DEGRADE_MAX_KSIZE = 25, FEMASR_DEGRADE_MAX_STRIDE = 4 };
+int femasr_degrade_mirror_conv(const float* x, float* y, int H, int W, const double* taps, int kh, int kw, int stride,
+                               int clip, void* stream);
+int femasr_degrade_resize_pass(const float* x, float* y, int H, int W, int axis, int out_n, const int* idx,
+                               const float* w, int K, int clip, void* stream);
+int femasr_degrade_noise_add(const float* x, const float* noise, int noise_ch, int H, int W, float* y, void* stream);
+/* 0 for sizes femasr_degrade_jpeg refuses */
+size_t femasr_degrade_jpeg_workspace_bytes(int H, int W);
+int femasr_degrade_jpeg(const float* x, float* y, int H, int W, const int* qtables, void* workspace,
+                        void* stream);
+
 /* layout helpers for tests */
 int femasr_nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, void* stream);
 int femasr_nhwc_to_nchw(const float* x, float* y, int B, int C, int H, int W, void* stream);
