@@ -16,9 +16,10 @@
 //              swizzled shared-memory stages into a register accumulator, then the epilogue from those registers
 //              (*2^-s + bias -> GELU -> + residual(s) -> fp32 NHWC or split-fp16 planes, GroupNorm partials, VQ top-4).
 // The ping-pong schedule (PP, 384 threads) gives the producer a warpgroup of its own and each consumer warpgroup whole
-// tiles, in turns on the tensor cores, so that one tile's epilogue runs under the next tile's MMAs.
-// The TMA epilogue (TMAE) of the cooperative BN-128 linears passes each finished tile through shared memory to TMA stores,
-// with the residual loaded by TMA, so that the consumers never wait on global memory.
+// tiles, in turns on the tensor cores, so that one tile's epilogue runs under the next tile's MMAs.  The cooperative F8
+// kernels (BN 128) have the same producer warpgroup, so that their consumers get 232 registers instead of 168.
+// The TMA epilogue (TMAE) of the cooperative BN-128 linears and F8 column-schedule convs passes each finished tile through
+// shared memory to TMA stores, with the residual loaded by TMA, so that the consumers never wait on global memory.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
@@ -84,6 +85,10 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // every committed store has finished reading its shared-memory source (the box may be rewritten)
@@ -225,8 +230,9 @@ constexpr int EPI_COLS = 32, EPI_BOX_BYTES = TC_BM * 128, EPI_BOXES = 2;
 
 // Shared memory: [COLS: activation column ring][stage ring][TMAE: epilogue boxes][barriers][GroupNorm partials].
 // Without COLS a stage holds all four operand boxes of a k-block; with COLS it holds the two weight boxes and the
-// activation columns have a ring of their own.  The TMA epilogue runs no GroupNorm partials: its boxes take their place
-// and it keeps 3 stages at BN 128 (3 x 65536 + 32768 + 1024 + 256 = 230656 bytes).
+// activation columns have a ring of their own.  The TMA epilogue of the linears runs no GroupNorm partials: its boxes take
+// their place and it keeps 3 stages at BN 128 (3 x 65536 + 32768 + 1024 + 256 = 230656 bytes).  The column-schedule
+// convs' boxes take one of their 4 weight stages (2 x 18432 x 2 + 3 x 32768 + 32768 + 1024 + 256 + 4096 = 210176 bytes).
 template <int BN, bool COLS = false, bool TMAE = false>
 struct TcCfg {
   static_assert(BN == 64 || BN == 128, "tile width");
@@ -234,14 +240,15 @@ struct TcCfg {
   static constexpr int STAGE_BYTES = (COLS ? 0 : 2 * A_PLANE_BYTES) + 2 * B_PLANE_BYTES;   // (a_hi, a_lo,) w_hi, w_lo
   static constexpr int COL_STAGES = COLS ? 2 : 0;
   static constexpr int COL_RING_BYTES = COL_STAGES * COL_STAGE_BYTES;
-  static constexpr int RED_BYTES = TMAE ? 0 : TC_CONSUMER_WARPS * 64 * 2 * 4;       // per-warp GroupNorm partials
+  static constexpr int RED_BYTES = TMAE && !COLS ? 0 : TC_CONSUMER_WARPS * 64 * 2 * 4;   // per-warp GroupNorm partials
   static constexpr int EPI_BYTES = TMAE ? EPI_BOXES * EPI_BOX_BYTES : 0;
-  // 3 (BN 128) / 4 (BN 64); COLS: 4 (BN 128) / 9 (BN 64); TMAE: 3
+  // 3 (BN 128) / 4 (BN 64); COLS: 4 (BN 128) / 9 (BN 64); TMAE: 3; COLS + TMAE: 3
   static constexpr int STAGES = (TC_SMEM_LIMIT - 1024 - 256 - RED_BYTES - COL_RING_BYTES - EPI_BYTES) / STAGE_BYTES;
   static constexpr int RING_BYTES = COL_RING_BYTES + STAGES * STAGE_BYTES + EPI_BYTES;
   static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + RED_BYTES;
   static constexpr int NF = BN / 2;                                                  // accumulator floats per thread
   static_assert(SMEM_BYTES <= TC_SMEM_LIMIT, "shared memory budget");
+  static_assert(!TMAE || STAGES == 3, "TMA epilogue: 3 stages beside the boxes");
   static_assert(16 * (STAGES + COL_STAGES) + 8 * (TMAE ? EPI_BOXES : 0) <= 256, "barrier area");
 };
 
@@ -456,8 +463,9 @@ __device__ __forceinline__ void walk_taps(const TcP& p, const Rings<Cfg>& r, Rin
 // PREFETCH_RES: the thread's residuals are all loaded before its first store.  As far as the compiler knows the stores
 // may alias res1 (they do in the in-place residual convs), so a load issued inside the store loop waits for the previous
 // stores and pays one memory round trip per column block and row; each element is still read before its own store.  The
-// ping-pong schedule prefetches.  The cooperative one loads inside the store loop: at BN 128 its 168 registers hold the
-// F8 / K-slice accumulator beside the tile's, and the prefetched residual spills.  Both compute the same values.
+// ping-pong schedule and the cooperative F8 kernels (232 registers beside a producer warpgroup) prefetch.  The other
+// cooperative kernels load inside the store loop: at BN 128 their 168 registers hold the K-slice accumulator beside the
+// tile's, and the prefetched residual spills.  Both compute the same values.
 template <int BN, bool RES, int EXT, bool PREFETCH_RES>
 __device__ __forceinline__ void epilogue_rows(const TcP& p, const TileCoord& tc, const float (&acc)[BN / 2], int row0,
                                               float inv_scale, float* red, int red_slot, int lane) {
@@ -550,19 +558,22 @@ __device__ __forceinline__ void gn_store_partials(const TcP& p, const TileCoord&
   named_bar_sync(bar, nthreads);
 }
 
-// ---------------------------------------------------------------- TMA epilogue (TMAE: cooperative BN-128 linears)
-// The output (fp32 y, or the hi and lo planes) and residual tensor maps: 2-D [tokens][Cout], boxes of 32 columns x 128
-// rows (tc_tma_epi_maps)
+// ---------------------------------------------------------------- TMA epilogue (TMAE: cooperative BN-128 linears and
+// F8 column-schedule convs)
+// The output (fp32 y, or the hi and lo planes) and residual tensor maps (tc_tma_epi_maps), boxes of 32 columns x 128 rows:
+// linears, 2-D [tokens][Cout]; CONV (column schedule), 4-D [B][H][W][Cout] in boxes of 32 ch x 8 cols x 16 rows x 1, whose
+// row order (y, then x) is the tile's accumulator row order.
 struct EpiMaps { const CUtensorMap *out0, *out1, *res; };
 
 // Residual column block s (columns 32 s .. 32 s + 31 of the tile) of tile tc into box s % 2 by TMA, completing on that
-// box's epi_full barrier.  Rows past the last token arrive as zeros and are never stored.
-template <class Cfg>
+// box's epi_full barrier.  Rows past the last token (CONV: outside the image) arrive as zeros and are never stored.
+template <bool CONV, class Cfg>
 __device__ __forceinline__ void load_res_block(const TcP& p, const Rings<Cfg>& r, const EpiMaps& e, const TileCoord& tc,
                                                int s) {
   const int b = s & 1;
   mbar_expect_tx(r.epi_full(b), EPI_BOX_BYTES);
-  tma_load_2d(r.epi(b), e.res, r.epi_full(b), tc.nt * 128 + EPI_COLS * s, tc.tx * p.Wt);
+  if constexpr (CONV) tma_load_4d(r.epi(b), e.res, r.epi_full(b), tc.nt * 128 + EPI_COLS * s, tc.tx * p.Wt, tc.ty * p.Ht, tc.b);
+  else tma_load_2d(r.epi(b), e.res, r.epi_full(b), tc.nt * 128 + EPI_COLS * s, tc.tx * p.Wt);
 }
 
 // The same rule per element as epilogue_rows (acc * 2^-s + bias -> GELU | ReLU -> + res1 -> fp32 or split_pack2), but
@@ -576,11 +587,22 @@ __device__ __forceinline__ void load_res_block(const TcP& p, const Rings<Cfg>& r
 // Bank conflicts: the split planes' 4-byte stores cover all 32 banks per warp.  The fp32 8-byte accesses are 2-way
 // conflicted (a half-warp spans 4 rows, so the swizzle spreads it over only 4 of the 8 chunks); permuting the column
 // blocks across lanes to avoid that costs the residual kernel spills at 168 registers.
-template <bool RES, class Cfg>
+// CONV (fp32 output only): the GroupNorm partials of the rows inside the image, from the same values, with the same sums
+// and shuffles as epilogue_rows, into red (the caller then runs gn_store_partials).
+template <bool RES, bool CONV, class Cfg>
 __device__ __forceinline__ void epilogue_tma(const TcP& p, const Rings<Cfg>& r, const EpiMaps& e, const TileCoord& tc,
-                                             int next, const float (&acc)[64], float inv_scale, int warp, int lane) {
+                                             int next, const float (&acc)[64], float inv_scale, float* red, int warp,
+                                             int lane) {
   const int rsub = lane >> 2, q = lane & 3;
   const int row = warp * 16 + rsub;                       // rows row and row + 8 of the tile
+  bool inside[2] = {true, true};
+  if constexpr (CONV) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int rr = row + 8 * h;
+      inside[h] = tc.ty * p.Ht + (rr >> p.wt_shift) < p.H && tc.tx * p.Wt + (rr & (p.Wt - 1)) < p.W;
+    }
+  }
   // fp32, 128B swizzle: (row, column 8 jj + 2 q) at row * 128 + (((2 jj + q / 2) ^ (row % 8)) << 4) + (q % 2) * 8,
   // i.e. 16-byte chunk 2 jj ^ f_x
   const uint32_t f_base = row * 128 + (q & 1) * 8;
@@ -588,12 +610,13 @@ __device__ __forceinline__ void epilogue_tma(const TcP& p, const Rings<Cfg>& r, 
   // split, 64B swizzle (per plane: 64-byte rows): row * 64 + ((jj ^ (row / 2 % 4)) << 4) + 4 q, i.e. chunk jj ^ h_x
   const uint32_t h_base = row * 64 + 4 * q;
   const int h_x = (row >> 1) & 3;
-  const bool split = p.out_hi != nullptr;
+  const bool split = !CONV && p.out_hi != nullptr;
   const int n0 = tc.nt * 128, row0 = tc.tx * p.Wt;
 #pragma unroll
   for (int s = 0; s < 4; ++s) {
     const int b = s & 1;
     const uint32_t box = r.epi(b);
+    float gs[4] = {0.f, 0.f, 0.f, 0.f}, gss[4] = {0.f, 0.f, 0.f, 0.f};   // CONV: the thread's two rows, per 8 columns
     if (RES) mbar_wait(r.epi_full(b), (uint32_t)(s >> 1));
     // row by row (h), so that only one row's residuals (8 registers) are live: at 168 registers more spills
 #pragma unroll
@@ -622,23 +645,45 @@ __device__ __forceinline__ void epilogue_tma(const TcP& p, const Rings<Cfg>& r, 
         } else {
           if (RES) { o.x += res[jj].x; o.y += res[jj].y; }
           sts_f2(box + f_base + 1024 * h + ((2 * jj ^ f_x) << 4), o);
+          if (CONV && inside[h]) { gs[jj] += o.x + o.y; gss[jj] = fmaf(o.x, o.x, fmaf(o.y, o.y, gss[jj])); }
+        }
+      }
+    }
+    if (CONV && p.gn_partial) {
+      // epilogue_rows' reduction, per 8 columns: over the warp's 16 rows (lanes sharing q), then over the lanes of a group
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+        for (int o = 4; o <= 16; o <<= 1) {
+          gs[jj] += __shfl_xor_sync(0xffffffffu, gs[jj], o); gss[jj] += __shfl_xor_sync(0xffffffffu, gss[jj], o);
+        }
+        if (p.cpg >= 4) { gs[jj] += __shfl_xor_sync(0xffffffffu, gs[jj], 1); gss[jj] += __shfl_xor_sync(0xffffffffu, gss[jj], 1); }
+        if (p.cpg >= 8) { gs[jj] += __shfl_xor_sync(0xffffffffu, gs[jj], 2); gss[jj] += __shfl_xor_sync(0xffffffffu, gss[jj], 2); }
+        if (rsub == 0 && (q & (p.cpg / 2 - 1)) == 0) {
+          const int g = (8 * (4 * s + jj) + 2 * q) / p.cpg;
+          red[(warp * 64 + g) * 2] = gs[jj];
+          red[(warp * 64 + g) * 2 + 1] = gss[jj];
         }
       }
     }
     fence_proxy_async_smem();
     if (threadIdx.x == 0) {
       bulk_wait_read_all();                               // the previous block's box (b ^ 1) is free
-      if (RES && (s == 1 || s == 2)) load_res_block(p, r, e, tc, s + 1);
-      if (RES && s == 3 && next >= 0) load_res_block(p, r, e, decode_tile(p, next), 0);
+      if (RES && (s == 1 || s == 2)) load_res_block<CONV>(p, r, e, tc, s + 1);
+      if (RES && s == 3 && next >= 0) load_res_block<CONV>(p, r, e, decode_tile(p, next), 0);
     }
     named_bar_sync(TC_EPI_BAR, 32 * TC_CONSUMER_WARPS);
     if (threadIdx.x == 0) {
-      tma_store_2d(e.out0, box, n0 + EPI_COLS * s, row0);
-      if (split) tma_store_2d(e.out1, box + EPI_BOX_BYTES / 2, n0 + EPI_COLS * s, row0);
+      if constexpr (CONV) {
+        tma_store_4d(e.out0, box, n0 + EPI_COLS * s, row0, tc.ty * p.Ht, tc.b);
+      } else {
+        tma_store_2d(e.out0, box, n0 + EPI_COLS * s, row0);
+        if (split) tma_store_2d(e.out1, box + EPI_BOX_BYTES / 2, n0 + EPI_COLS * s, row0);
+      }
       bulk_commit();
       if (RES && s == 3 && next >= 0) {
         bulk_wait_read_all();                             // box 1 read out: the next tile's block 1 loads under its k-loop
-        load_res_block(p, r, e, decode_tile(p, next), 1);
+        load_res_block<CONV>(p, r, e, decode_tile(p, next), 1);
       }
     }
   }
@@ -658,10 +703,13 @@ __device__ __forceinline__ void epilogue_tma(const TcP& p, const Rings<Cfg>& r, 
 // the two take turns on the tensor cores, and one runs its epilogue while the other runs its k-loop (plan_tiles).
 // Both schedules issue their k-blocks through mma_kblock, walk the rings with walk_columns / walk_taps and store through
 // epilogue_rows and gn_store_partials; they differ in how many k-blocks stay in flight and where a stage is released.
-// TMAE: the cooperative BN-128 linears (1x1, no F8, no GroupNorm partials, no res2) store through epilogue_tma and the
-// output / residual maps map_o0, map_o1, map_r (unused otherwise), instead of from registers (plan_tiles).
+// The F8 kernels all run with a producer warpgroup (PWG, TC_PP_THREADS): the cooperative ones (BN 128) then have 232
+// registers per consumer thread for the F8 accumulator beside the tile's and the prefetched residual.
+// TMAE: the cooperative BN-128 linears (1x1, no F8, no GroupNorm partials, no res2) and the F8 column-schedule convs (fp32
+// output, no res2) store through epilogue_tma and the output / residual maps map_o0, map_o1, map_r (unused otherwise),
+// instead of from registers (plan_tiles).
 template <int BN, bool RES, bool F8, bool VQ = false, int EXT = 0, bool COLS = false, bool PP = false, bool TMAE = false>
-__global__ void __launch_bounds__(PP ? TC_PP_THREADS : TC_THREADS, 1)
+__global__ void __launch_bounds__(PP || F8 ? TC_PP_THREADS : TC_THREADS, 1)
 tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                 const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const TcP p,
                 const __grid_constant__ CUtensorMap map_o0, const __grid_constant__ CUtensorMap map_o1,
@@ -671,7 +719,9 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
   static_assert(!VQ || (!RES && !F8), "VQ mode: plain linear tiles");
   static_assert(!COLS || (F8 && !VQ && EXT == 0), "column schedule: F8 3x3 convs");
   static_assert(!PP || (BN == 64 && !VQ), "ping-pong schedule: BN-64 convs and linears");
-  static_assert(!TMAE || (BN == 128 && !F8 && !VQ && EXT == 0 && !COLS && !PP), "TMA epilogue: cooperative BN-128 linears");
+  static_assert(!TMAE || (BN == 128 && F8 == COLS && !VQ && EXT == 0 && !PP),
+                "TMA epilogue: cooperative BN-128 linears and F8 column-schedule convs");
+  constexpr bool PWG = PP || F8;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const Rings<Cfg> r{smem_base, smem_base + Cfg::RING_BYTES};
@@ -688,8 +738,8 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
   }
   __syncthreads();
 
-  if (PP ? warp >= TC_CONSUMER_WARPS : warp == TC_CONSUMER_WARPS) {
-    if constexpr (PP) {
+  if (PWG ? warp >= TC_CONSUMER_WARPS : warp == TC_CONSUMER_WARPS) {
+    if constexpr (PWG) {
       setmaxnreg_dec<PP_PRODUCER_REGS>();      // the whole warpgroup; one lane of its first warp issues the loads
       if (warp != TC_CONSUMER_WARPS) return;
     }
@@ -764,6 +814,7 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
   }
 
   // ===================== cooperative consumers: two warpgroups x 64 accumulator rows =====================
+  if constexpr (PWG) setmaxnreg_inc<PP_CONSUMER_REGS>();
   const int rsub = lane >> 2, q = lane & 3;
   const uint32_t a_off = wg * (A_PLANE_BYTES / 2);  // this warpgroup's 64 rows of the A operand
   const int slice_len = p.slice_kb > 0 ? p.slice_kb : (p.kb_end - p.kb_begin);
@@ -777,8 +828,8 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
 
   if (TMAE && RES && threadIdx.x == 0 && work_of<false>(p, 0) >= 0) {
     const TileCoord tc = decode_tile(p, work_of<false>(p, 0));     // the first tile's residual blocks 0 and 1
-    load_res_block(p, r, EpiMaps{&map_o0, &map_o1, &map_r}, tc, 0);
-    load_res_block(p, r, EpiMaps{&map_o0, &map_o1, &map_r}, tc, 1);
+    load_res_block<COLS>(p, r, EpiMaps{&map_o0, &map_o1, &map_r}, tc, 0);
+    load_res_block<COLS>(p, r, EpiMaps{&map_o0, &map_o1, &map_r}, tc, 1);
   }
 
   for (int it = 0, work; (work = work_of<VQ>(p, it)) >= 0; ++it) {
@@ -858,11 +909,13 @@ tc_igemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_const
       continue;
     }
     if constexpr (TMAE) {
-      epilogue_tma<RES>(p, r, EpiMaps{&map_o0, &map_o1, &map_r}, tc, work_of<false>(p, it + 1), acc[0], inv_scale, warp, lane);
+      epilogue_tma<RES, COLS>(p, r, EpiMaps{&map_o0, &map_o1, &map_r}, tc, work_of<false>(p, it + 1), acc[0], inv_scale,
+                              red, warp, lane);
+      if (COLS && p.gn_partial) gn_store_partials<BN>(p, tc, red, 64, threadIdx.x, 32 * TC_CONSUMER_WARPS, TC_GN_BAR);
       continue;
     }
     // 16-row group `warp` of the tile
-    epilogue_rows<BN, RES, EXT, false>(p, tc, acc[0], warp * 16, inv_scale, red, warp * 64, lane);
+    epilogue_rows<BN, RES, EXT, PWG>(p, tc, acc[0], warp * 16, inv_scale, red, warp * 64, lane);
     if (p.gn_partial) gn_store_partials<BN>(p, tc, red, 64, threadIdx.x, 32 * TC_CONSUMER_WARPS, TC_GN_BAR);
   }
   if (TMAE && threadIdx.x == 0) bulk_wait_all();    // the tile stores complete before the CTA exits
@@ -1252,7 +1305,17 @@ static int make_maps(TcMaps* m, const void* a_hi, const void* a_lo, int B, int H
 // The TMA epilogue's maps over the 1x1 launch's token row ([tokens][Cout], tokens = p.W): fp32 y (or the split hi and
 // lo planes) and res1, boxes of 32 columns x 128 rows = 128-byte rows (fp32: 128B swizzle; fp16 planes: 64-byte rows,
 // 64B swizzle), matching epilogue_tma's shared-memory layout.  The store clips the rows past the last token.
-static int tc_tma_epi_maps(TcMaps* m, const TcP& p) {
+// Column-schedule convs: fp32 y and res1 over the NHWC output [B][H][W][Cout] in 4-D boxes of 32 ch x 8 cols x 16 rows
+// x 1, the same 128 rows of 128 bytes; the store clips the pixels outside the image.
+static int tc_tma_epi_maps(TcMaps* m, const TcP& p, bool cols) {
+  if (cols) {
+    const cuuint64_t dims[4] = {(cuuint64_t)p.Cout, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.B};
+    const cuuint64_t str[3] = {(cuuint64_t)p.Cout * 4, (cuuint64_t)p.W * p.Cout * 4, (cuuint64_t)p.H * p.W * p.Cout * 4};
+    const cuuint32_t box[4] = {(cuuint32_t)EPI_COLS, (cuuint32_t)COL_WT, (cuuint32_t)COL_HT, 1};
+    int s = make_map(&m->o0, p.y, 4, dims, str, box, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
+    if (!s && p.res1) s = make_map(&m->res, p.res1, 4, dims, str, box, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
+    return s;
+  }
   const cuuint64_t dims[2] = {(cuuint64_t)p.Cout, (cuuint64_t)p.W};
   const cuuint32_t box[2] = {(cuuint32_t)EPI_COLS, (cuuint32_t)TC_BM};
   const cuuint64_t str32[1] = {(cuuint64_t)p.Cout * 4}, str16[1] = {(cuuint64_t)p.Cout * 2};
@@ -1277,7 +1340,7 @@ static int launch_tc_v(const TcMaps& m, const TcP& p, cudaStream_t st) {
   }
   const int items = VQ ? p.num_tiles / p.n_tiles : p.num_tiles;     // VQ: one CTA walks all code tiles of an m-tile
   const int grid = items < sm_count() ? items : sm_count();
-  tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP, TMAE><<<grid, PP ? TC_PP_THREADS : TC_THREADS, Cfg::SMEM_BYTES, st>>>(
+  tc_igemm_kernel<BN, RES, F8, VQ, EXT, COLS, PP, TMAE><<<grid, PP || F8 ? TC_PP_THREADS : TC_THREADS, Cfg::SMEM_BYTES, st>>>(
       m.a_hi, m.a_lo, m.b_hi, m.b_lo, p, m.o0, m.o1, m.res);
   return launch_status(VQ ? "tc_igemm_kernel(vq)" : "tc_igemm_kernel");
 }
@@ -1331,7 +1394,9 @@ static void tc_tile_shape(int H, int W, int* Wt, int* Ht) {
 // The TMA epilogue (tc_igemm_kernel's TMAE) runs the cooperative BN-128 1x1 launches without F8, GroupNorm partials,
 // res2 or LeakyReLU, and without a residual beside a split output (the Swin linears, the 1x1s before the VQ, the im2col
 // first-conv GEMM at Cout 128 / 256, conv_semantic): their short k-loops left the tensor cores idle while the register
-// epilogue waited on global memory.
+// epilogue waited on global memory.  It also runs the BN-128 column-schedule convs with an fp32 output and no res2 (the
+// 3x3 convs behind the VQ at 128 and 256 channels), whose register epilogue stalled the tensor cores on the in-place
+// residual's loads.  The res2 launches (2 per forward) and the upsample convs keep the register epilogue.
 struct TilePlan { int Wt, Ht, wt_shift, tiles_x, tiles_y, BN; bool cols, pingpong, tma_epilogue; };
 static TilePlan plan_tiles(const femasr_tc_args* a, int H, int W, bool sliced = false) {
   TilePlan t;
@@ -1347,8 +1412,8 @@ static TilePlan plan_tiles(const femasr_tc_args* a, int H, int W, bool sliced = 
   // 16-byte aligned outputs and residual: the TMA maps' global addresses
   auto al16 = [](const void* q) { return ((uintptr_t)q & 15u) == 0; };
   const bool split = a->out_hi != nullptr;
-  t.tma_epilogue = t.BN == 128 && !t.pingpong && !t.cols && a->ksize == 1 && !a->f8 && !a->gn_partial &&
-                   !a->res2 && a->act != FEMASR_ACT_LRELU && !(split && a->res1) &&
+  t.tma_epilogue = t.BN == 128 && !t.pingpong && !a->res2 &&
+                   (t.cols ? !split : a->ksize == 1 && !a->f8 && !a->gn_partial && a->act != FEMASR_ACT_LRELU && !(split && a->res1)) &&
                    (split ? al16(a->out_hi) && al16(a->out_lo) : al16(a->y)) && (!a->res1 || al16(a->res1));
   return t;
 }
@@ -1595,8 +1660,11 @@ extern "C" int femasr_tc_igemm(const femasr_tc_args* a, void* stream) {
   if (s) return s;
   cudaStream_t st = as_stream(stream);
   if (plan.tma_epilogue) {
-    const int se = tc_tma_epi_maps(&m, p);
+    const int se = tc_tma_epi_maps(&m, p, plan.cols);
     if (se) return se;
+    if (plan.cols)
+      return p.res1 ? launch_tc_v<128, true, true, false, 0, true, false, true>(m, p, st)
+                    : launch_tc_v<128, false, true, false, 0, true, false, true>(m, p, st);
     return p.res1 ? launch_tc_v<128, true, false, false, 0, false, false, true>(m, p, st)
                   : launch_tc_v<128, false, false, false, 0, false, false, true>(m, p, st);
   }

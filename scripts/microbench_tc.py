@@ -30,8 +30,10 @@ F8 = int(os.environ.get('MB_F8', '0'))      # 1: the 3x3 convs in the F8 cross-t
 GN = int(os.environ.get('MB_GN', '0'))      # 1: the 3x3 convs also emit GroupNorm partial sums (what most of them do in the network)
 
 
-def conv_case(name, B, H, W, Cin, Cout, ksize=3, up=0, res=False, act=0, split=False, bias=True, slice_kb=0, inplace=False):
-    """inplace: the output overwrites the residual (y = res1), as proj and fc2 do in the network."""
+def conv_case(name, B, H, W, Cin, Cout, ksize=3, up=0, res=False, act=0, split=False, bias=True, slice_kb=0, inplace=False,
+              res2=False):
+    """inplace: the output overwrites the residual (y = res1), as proj, fc2 and the ResBlocks' second convs do in the
+    network; res2: a second residual, as the last conv of decoder blocks 0 and 1 adds."""
     if ONLY and not any(o in name for o in ONLY.split('|')):
         return 0.0
     hi = (torch.randn(B, H, W, Cin, device=dev) * 0.5).half()
@@ -48,10 +50,12 @@ def conv_case(name, B, H, W, Cin, Cout, ksize=3, up=0, res=False, act=0, split=F
     r = torch.randn(B, H * u, W * u, Cout, device=dev) if res else None
     if inplace:
         y = r
+    r2 = torch.randn(B, H * u, W * u, Cout, device=dev) if res2 else None
     gn = None
     if GN and ksize == 3 and not split:
         gn = torch.empty(B * G.tc_gn_rows(B, H, W, Cin, Cout, upsample=up, slice_kb=slice_kb) * 64, device=dev)
-    fn = lambda: G.tc_igemm(hi, lo, blob, b, Cout, ksize, act=act, res1=r, y=y, upsample=up, split_out=split, slice_kb=slice_kb, f8=f8, gn_partial=gn)
+    fn = lambda: G.tc_igemm(hi, lo, blob, b, Cout, ksize, act=act, res1=r, res2=r2, y=y, upsample=up, split_out=split,
+                            slice_kb=slice_kb, f8=f8, gn_partial=gn)
     ms = timeit(fn)
     flops = 2.0 * B * H * u * W * u * Cout * Cin * ksize * ksize
     execd = (2 if f8 else 3) * 2.0 * B * H * W * Cout * Cin * (4 * 4 if up else ksize * ksize)
@@ -72,8 +76,14 @@ conv_case("fc2 1024->256 +res sliced in place", 32, 64, 64, 1024, 256, 1, res=Tr
 conv_case("conv 256->256 @64x64 +res sliced", 32, 64, 64, 256, 256, res=True, slice_kb=4)
 print("# 3x3 convs, batch 32")
 conv_case("conv 256->256 @64x64 +res", 32, 64, 64, 256, 256, res=True)
+conv_case("conv 256->256 @128x128", 32, 128, 128, 256, 256)
 conv_case("conv 256->256 @128x128 +res", 32, 128, 128, 256, 256, res=True)
+conv_case("conv 256->256 @128x128 +res in place", 32, 128, 128, 256, 256, res=True, inplace=True)
+conv_case("conv 256->256 @128x128 +res in place +res2", 32, 128, 128, 256, 256, res=True, inplace=True, res2=True)
+conv_case("conv 128->128 @256x256", 32, 256, 256, 128, 128)
 conv_case("conv 128->128 @256x256 +res", 32, 256, 256, 128, 128, res=True)
+conv_case("conv 128->128 @256x256 +res in place", 32, 256, 256, 128, 128, res=True, inplace=True)
+conv_case("conv 128->128 @256x256 +res in place +res2", 32, 256, 256, 128, 128, res=True, inplace=True, res2=True)
 conv_case("conv 64->64 @512x512 +res", 32, 512, 512, 64, 64, res=True)
 conv_case("conv 64->64 @512x512", 32, 512, 512, 64, 64)
 print("# upsample-fused (sub-pixel) convs, low-res input size given")
