@@ -83,16 +83,19 @@ struct Arena {
 
 
 // The device forms femasr_net_set_param packs a parameter into, besides its fp32 copy in the reference layout.  The spec
-// decides them once from the layer's role and the net's configuration; the graph reads the same flags.
+// decides them once from the layer's role, its shape and the net's gemm_path: exactly the forms a launch on that path
+// reads.  The graph reads the same flags.
 constexpr unsigned
-  FORM_KMAJOR = 1u << 0,   // K-major fp32 GEMM operand (conv / linear weight; codebook^T): the SIMT GEMM's weight
+  FORM_KMAJOR = 1u << 0,   // K-major fp32 GEMM operand (conv / linear weight; codebook^T): the SIMT GEMM's weight, and
+                           // the weight of the in_conv, out_conv and conv9 kernels
   FORM_TC = 1u << 1,       // split-fp16 blob: the tensor-core GEMM's weight (codebook: the fused VQ's B operand)
   FORM_TC8 = 1u << 2,      // the same in the F8 cross-term packing (3x3 convs that may run behind the VQ)
   FORM_UP = 1u << 3,       // sub-pixel phase filters of a nearest-x2 -> conv3x3 site, split fp16
   FORM_UP8 = 1u << 4,      // the same in the F8 packing
   FORM_IM2COL = 1u << 5,   // [Cout][kpad] zero-padded im2col matrix (in_conv, VGG conv1_1, AlexNet conv1; kpad = im2col_k):
                            // split-fp16 blob on gemm_path 1, K-major fp32 on gemm_path 0
-  FORM_RELB = 1u << 6,     // rel-pos table expanded to [8][64][64] (SIMT attention) and in the mma kernel's fragment order
+  FORM_RELB = 1u << 6,     // rel-pos table expanded to [8][64][64] (SIMT attention, gemm_path 0) or in the mma kernel's
+                           // fragment order (gemm_path 1)
   FORM_ESQ = 1u << 7;      // sum e^2 per codebook row
 
 struct ParamInfo {
@@ -105,13 +108,12 @@ struct ParamInfo {
 // every device buffer of one parameter; nullptr where its ParamInfo lists no such form
 struct DevParam {
   float* raw = nullptr;        // fp32 copy in the reference layout
-  float* packed = nullptr;     // FORM_KMAJOR, or the expanded rel bias of FORM_RELB
-  float* relb_mma = nullptr;   // FORM_RELB, fragment order
+  float* packed = nullptr;     // FORM_KMAJOR, or the rel bias of FORM_RELB in the layout of the net's gemm_path
   float* esq = nullptr;        // FORM_ESQ
   void *tc = nullptr, *tc8 = nullptr, *up = nullptr, *up8 = nullptr, *im2col = nullptr;
   float* sigma = nullptr;      // spectral-norm weight_orig: {u . (W v), |W v|} (femasr_spectral_sigma); the forms above
   float sn[2] = {0.f, 0.f};    // are packed from weight_orig / sigma.  sn: the same two values on the host
-  void release() { for (void* p : {(void*)raw, (void*)packed, (void*)relb_mma, (void*)esq, tc, tc8, up, up8, im2col, (void*)sigma}) cudaFree(p); }
+  void release() { for (void* p : {(void*)raw, (void*)packed, (void*)esq, tc, tc8, up, up8, im2col, (void*)sigma}) cudaFree(p); }
 };
 
 struct Tap { float* dst; size_t cap; };
@@ -155,13 +157,7 @@ struct femasr_net {
   int last_launches = 0;
   bool profile = false;
   int poison = -1;                        // femasr_net_set_poison: byte every workspace block is filled with, -1 = off
-  bool tc_precise = true;                 // K-sliced fp32 accumulation for the layers in front of the VQ
-  bool f8_cross = true;                   // layers behind the VQ: the two cross products of the split as one fp8 product (FEMASR_F8_CROSS=0: three fp16 products)
-  int tc_slice_kb = 4;                    // K-slice length in 64-wide k-blocks (FEMASR_TC_SLICE_KB; study knob)
-  bool vq_fused = true;                   // VQ distances on the tensor cores with the argmin fused (FEMASR_VQ_FUSED=0: fp32 SIMT z.E^T + vq_select)
-  bool fast_silu = true;                  // approximate-unit SiLU in the operand staging behind the VQ (FEMASR_FAST_SILU=0: exact)
   bool semantic = false;                  // femasr_net_enable_semantic: the VGG19 / conv_semantic tensors are part of the spec
-  int sem_slice_kb = 0;                   // K-slice length of the semantic branch's GEMMs (FEMASR_SEM_SLICE_KB; study knob, 0 = one pass)
   bool disc = false;                      // femasr_disc_create: a UNetDiscriminatorSN (dcfg); cfg holds only gemm_path
   femasr_disc_config dcfg{};
   bool lpips = false;                     // femasr_lpips_create: an LPIPS metric (lcfg); cfg holds only gemm_path
@@ -191,15 +187,18 @@ static int chan(int res) {
 // DISC_CONV: a discriminator conv (spectral-norm 3x3 or 4x4 stride 2), never F8
 enum Role { CONV, UP_CONV, IN_CONV, VGG_CONV, VGG_CONV1, DISC_CONV };
 
+// The forms the launches of a conv / linear weight read on the net's gemm_path.  VGG_CONV1 is an im2col GEMM on both
+// paths.  gemm_path 0 runs the rest on the SIMT GEMM and the in_conv / head kernels.  On gemm_path 1 the tensor-core GEMM
+// takes every shape it tiles, an up conv always with its upsample fused; in_conv keeps the K-major weight for the fp32
+// in_conv its tap runs, and the out_conv / conv9 heads (Cout 3 / 1) theirs.
 static unsigned weight_forms(const femasr_net* n, Role r, int ci, int co, int k) {
-  const bool tc = n->cfg.gemm_path == 1;
-  if (r == VGG_CONV1 || (r == IN_CONV && tc)) return FORM_KMAJOR | FORM_IM2COL;   // K = 27 / 48 -> 64, 363 -> 384
-  if (!tc || (k != 1 && k != 3 && k != 4 && k != 5) || ci % 64 || co % 64) return FORM_KMAJOR;
-  unsigned f = FORM_KMAJOR | FORM_TC;
-  if (n->f8_cross && k == 3 && r != VGG_CONV && r != DISC_CONV) f |= FORM_TC8;   // may run behind the VQ; the VGG and
-                                                                                  // discriminator convs never use F8
-  if (r == UP_CONV) f |= FORM_UP | (n->f8_cross ? FORM_UP8 : 0);
-  return f;
+  if (r == VGG_CONV1) return FORM_IM2COL;                                         // K = 27 -> 64, 363 -> 384
+  if (n->cfg.gemm_path == 0) return FORM_KMAJOR;
+  if (r == IN_CONV) return FORM_KMAJOR | FORM_IM2COL;                             // K = 48 -> 64
+  if ((k != 1 && k != 3 && k != 4 && k != 5) || ci % 64 || co % 64) return FORM_KMAJOR;
+  if (r == UP_CONV) return FORM_UP | FORM_UP8;
+  // F8 for the 3x3 convs that may run behind the VQ; the VGG and discriminator convs never use it
+  return FORM_TC | (k == 3 && r != VGG_CONV && r != DISC_CONV ? FORM_TC8 : 0);
 }
 static void add_conv(femasr_net* n, const std::string& p, int ci, int co, int k, Role r = CONV) {
   n->spec[p + ".weight"] = ParamInfo{(size_t)co * ci * k * k, co, ci, k, weight_forms(n, r, ci, co, k)};
@@ -252,7 +251,8 @@ static void build_spec(femasr_net* n) {
   }
   for (int i = 0; i < 3; ++i) add_up_block(n, "decoder_group." + std::to_string(i) + ".block", chan(32 << i), chan(64 << i));
   add_conv(n, "out_conv", 64, 3, 3);
-  const unsigned cb_forms = FORM_KMAJOR | FORM_ESQ | (n->cfg.gemm_path == 1 && n->vq_fused ? FORM_TC : 0);
+  // codebooks: the fused tensor-core VQ on gemm_path 1, the fp32 SIMT z.E^T + vq_select on gemm_path 0
+  const unsigned cb_forms = FORM_ESQ | (n->cfg.gemm_path == 1 ? FORM_TC : FORM_KMAJOR);
   for (size_t k = 0; k < n->cbs.size(); ++k) {           // femasr_arch.py:280-299
     const femasr_net::Codebook& cb = n->cbs[k];
     const std::string ks = std::to_string(k);
@@ -461,9 +461,13 @@ struct Ctx {
     if (it == net->dev.end()) { check(fail(FEMASR_ERR_STATE, "parameter not set: " + name)); return none; }
     return it->second;
   }
-  const float* P(const std::string& name) {      // packed (or raw when there is no packed form)
-    const DevParam& d = D(name);
-    return d.packed ? d.packed : d.raw;
+  // a tensor without device forms (bias, norm, vector): its fp32 copy
+  const float* P(const std::string& name) { return D(name).raw; }
+  // the FORM_KMAJOR / FORM_RELB form of a weight a dedicated kernel reads; a weight the spec did not pack so fails the run
+  const float* packed(const std::string& name) {
+    const float* p = D(name).packed;
+    if (!dry() && !p) check(fail(FEMASR_ERR_STATE, "parameter not packed: " + name));
+    return p;
   }
   bool has(const std::string& name, unsigned form) const { return (net->spec.at(name).forms & form) != 0; }
   bool tapped(const char* stage) const {
@@ -510,21 +514,21 @@ struct Ctx {
     return net->cfg.gemm_path == 1 && (d.im2col || has(d.wname(), d.upsample ? FORM_UP : FORM_TC));
   }
 
-  // The numerics policy.  In front of the VQ (index-critical): every tc_slice_kb k-blocks the tensor core's truncating
+  // The numerics policy.  In front of the VQ (index-critical): every SLICE_KB k-blocks the tensor core's truncating
   // accumulator is folded into an fp32 round-to-nearest running sum (see femasr_tc_args.slice_kb).  Behind it (bar: 1e-3
   // on the output): approximate-unit SiLU, and the two cross products of the split as one fp8 product.  The semantic
-  // branch runs in one pass (or FEMASR_SEM_SLICE_KB) without F8, wherever in the graph it sits.
+  // branch runs in one pass without F8, wherever in the graph it sits.
+  static constexpr int SLICE_KB = 4;
   Numerics numerics(const ConvDesc& d) const {
     Numerics m;
     m.prologue = d.pro;
-    if (d.semantic) {
-      m.slice_kb = net->sem_slice_kb;
-    } else if (precise_region) {
+    if (d.semantic) return m;
+    if (precise_region) {
       const int nkb = (d.upsample ? 4 : d.k * d.k) * (d.Cin / 64);
-      if (net->tc_precise && nkb > net->tc_slice_kb) m.slice_kb = net->tc_slice_kb;
+      if (nkb > SLICE_KB) m.slice_kb = SLICE_KB;
     } else {
       m.f8 = !d.a_hi && d.k == 3 && d.pro != FEMASR_PRO_LN && has(d.wname(), d.upsample ? FORM_UP8 : FORM_TC8);
-      if (d.pro == FEMASR_PRO_GN_SILU && net->fast_silu) m.prologue = FEMASR_PRO_GN_SILU_FAST;
+      if (d.pro == FEMASR_PRO_GN_SILU) m.prologue = FEMASR_PRO_GN_SILU_FAST;
     }
     return m;
   }
@@ -720,6 +724,7 @@ struct Ctx {
         f1.x = T; f1.pro = FEMASR_PRO_LN; f1.gamma = P(bp + ".norm2.weight"); f1.beta = P(bp + ".norm2.bias");
         f1.act = FEMASR_ACT_GELU;
         f2.y = T; f2.res1 = T;
+        const float* rb = packed(rbname);
         if (tc) {
           // operands travel between the kernels as split fp16 planes: `ao` and `hid` are reinterpreted as
           // [hi plane | lo plane] (same byte size as the fp32 tensors they replace); LayerNorm runs in the staging
@@ -727,15 +732,13 @@ struct Ctx {
           __half* hd_hi = reinterpret_cast<__half*>(hid); __half* hd_lo = hd_hi + M * 4 * C;
           o.a_hi = ao_hi; o.a_lo = ao_lo; f1.o_hi = hd_hi; f1.o_lo = hd_lo; f2.a_hi = hd_hi; f2.a_lo = hd_lo;
           conv(q);
-          const float* rbm = D(rbname).relb_mma;
           run("window_attention_mma", attn_flops, [&] {
-            return femasr_window_attention_mma(qkv, rbm, nullptr, ao_hi, ao_lo, B, H, W, C, 8, (b & 1) ? 4 : 0, st);
+            return femasr_window_attention_mma(qkv, rb, nullptr, ao_hi, ao_lo, B, H, W, C, 8, (b & 1) ? 4 : 0, st);
           });
           conv(o); conv(f1); conv(f2);
           continue;
         }
         q.pa = f1.pa = mu; q.pb = f1.pb = rs; o.x = ao; f1.y = hid; f2.x = hid;
-        const float* rb = P(rbname);
         run("ln_stats", 0.0, [&] { return femasr_ln_stats(in, mu, rs, (int)M, C, 1e-5f, st); });
         conv(q);
         run("window_attention", attn_flops,
@@ -884,7 +887,8 @@ struct Ctx {
     tap(k == 0 ? "z" : (k == 1 ? "z1" : "z2"), z, N * e);
     const std::string cname = "quantize_group." + ks + ".embedding.weight";
     const bool fused = has(cname, FORM_TC);
-    // fused: tensor-core distances + in-kernel top-4 (no [N, n_e] tensor); else the fp32 SIMT product + vq_select
+    // fused (gemm_path 1): tensor-core distances + in-kernel top-4 (no [N, n_e] tensor); else the fp32 SIMT product +
+    // vq_select
     float *zc = nullptr, *arow = nullptr, *zhi = nullptr, *zlo = nullptr, *cand = nullptr;
     if (fused) {
       arow = ar.alloc(N);
@@ -999,7 +1003,7 @@ struct Ctx {
       tap(i == 0 ? "dec0" : (i == 1 ? "dec1" : "dec2"), t, (size_t)B * 2 * hh * 2 * ww * co);
     }
     if (prev_q) { ar.release(prev_q); ar.release(prev_z); }
-    const float *ow = P("out_conv.weight"), *ob = P("out_conv.bias");
+    const float *ow = packed("out_conv.weight"), *ob = P("out_conv.bias");
     const float* d2 = t;
     run("out_conv", 2.0 * 9 * 64 * 3 * (double)B * 64 * h * w,
         [&] { return net->cfg.gemm_path == 1 ? femasr_out_conv3x3_mma(d2, ow, ob, y_nchw, B, 8 * h, 8 * w, 64, st)
@@ -1016,12 +1020,12 @@ struct Ctx {
     const bool tc = cfg.gemm_path == 1;
     if (sem_loss) semantic_vgg(x_nchw, B, H, W);
     precise_region = true;
-    const float *iw = P(enc + ".in_conv.weight"), *ib = P(enc + ".in_conv.bias");
     float* cur = nullptr;                 // fp32 in_conv output (SIMT path, or when its tap is requested)
     Operand in_split;                     // tensor-core path: in_conv writes the down conv's split operand planes directly
     const size_t in_elems = (size_t)B * h * w * c;
     if (!tc || tapped("in_conv")) {       // identical in the sizing run and the real run: taps are registered first
       cur = ar.alloc(in_elems);
+      const float *iw = packed(enc + ".in_conv.weight"), *ib = P(enc + ".in_conv.bias");
       const int c0 = c;
       run("in_conv", 2.0 * 16 * cfg.in_channel * c * (double)B * h * w,
           [&] { return femasr_in_conv4x4(x_nchw, iw, ib, cur, B, cfg.in_channel, H, W, c0, st); });
@@ -1142,7 +1146,7 @@ struct Ctx {
     release(o);
     conv(g8.in(q).out(Operand{x8}));
     release(q);
-    const float *w9 = P("conv9.weight"), *b9 = P("conv9.bias");
+    const float *w9 = packed("conv9.weight"), *b9 = P("conv9.bias");
     run("disc_head", 2.0 * 9 * F * (double)B * H * W,
         [&] { return femasr_out_conv3x3_n(x8, w9, b9, y_nchw, B, H, W, F, 1, tc ? 1 : 0, st); });
     ar.release(x8);
@@ -1232,8 +1236,8 @@ static int pack_forms(femasr_net* net, DevParam& d, const ParamInfo& pi, const f
   if ((f & FORM_UP) && ((s = ensure(&d.up, upb)) || (s = femasr_tc_pack_weight_up2(src, d.up, co, ci, st)))) return s;
   if ((f & FORM_UP8) && ((s = ensure(&d.up8, upb)) || (s = femasr_tc_pack_weight_up2_f8(src, d.up8, co, ci, st)))) return s;
   if ((f & FORM_RELB) &&
-      ((s = ensure(&d.packed, 8 * 64 * 64 * sizeof(float))) || (s = ensure(&d.relb_mma, 8 * 64 * 64 * sizeof(float))) ||
-       (s = femasr_expand_rel_bias_mma(src, d.relb_mma, 8, st)) || (s = femasr_expand_rel_bias(src, d.packed, 8, st))))
+      ((s = ensure(&d.packed, 8 * 64 * 64 * sizeof(float))) ||
+       (s = net->cfg.gemm_path == 1 ? femasr_expand_rel_bias_mma(src, d.packed, 8, st) : femasr_expand_rel_bias(src, d.packed, 8, st))))
     return s;
   if ((f & FORM_ESQ) && ((s = ensure(&d.esq, co * sizeof(float))) || (s = femasr_row_sumsq(src, d.esq, co, ci, st)))) return s;
   return FEMASR_OK;
@@ -1267,16 +1271,6 @@ static int check_disc_geometry(int B, int H, int W) {
     return fail(FEMASR_ERR_ARG, "disc: H and W must be multiples of 8 (three stride-2 convs, then x2 upsamples that must "
                                 "meet the skip tensors; the reference raises at the skip add)");
   return FEMASR_OK;
-}
-
-// Study knobs read from the environment at create time (every kind of handle)
-static void read_knobs(femasr_net* n) {
-  if (const char* ev = getenv("FEMASR_TC_PRECISE")) n->tc_precise = atoi(ev) != 0;
-  if (const char* ev = getenv("FEMASR_FAST_SILU")) n->fast_silu = atoi(ev) != 0;
-  if (const char* ev = getenv("FEMASR_VQ_FUSED")) n->vq_fused = atoi(ev) != 0;
-  if (const char* ev = getenv("FEMASR_F8_CROSS")) n->f8_cross = atoi(ev) != 0;
-  if (const char* ev = getenv("FEMASR_TC_SLICE_KB")) n->tc_slice_kb = std::max(1, atoi(ev));
-  if (const char* ev = getenv("FEMASR_SEM_SLICE_KB")) n->sem_slice_kb = std::max(0, atoi(ev));
 }
 
 }  // namespace femasr
@@ -1322,7 +1316,6 @@ extern "C" int femasr_net_create(const femasr_net_config* cfg, femasr_net** out)
   }
   n->depth = cfg->scale_factor == 4 ? 1 : (cfg->scale_factor == 2 ? 2 : 3);
   n->hq = cfg->scale_factor == 1;
-  read_knobs(n);
   build_spec(n);
   *out = n;
   return FEMASR_OK;
@@ -1547,7 +1540,6 @@ extern "C" int femasr_disc_create(const femasr_disc_config* cfg, femasr_net** ou
   n->cfg.gemm_path = cfg->gemm_path;
   n->disc = true;
   n->dcfg = *cfg;
-  read_knobs(n);
   build_disc_spec(n);
   *out = n;
   return FEMASR_OK;
@@ -1623,7 +1615,6 @@ extern "C" int femasr_lpips_create(const femasr_lpips_config* cfg, femasr_net** 
   n->cfg.gemm_path = cfg->gemm_path;
   n->lpips = true;
   n->lcfg = *cfg;
-  read_knobs(n);
   build_lpips_spec(n);
   *out = n;
   return FEMASR_OK;

@@ -1,12 +1,15 @@
 #!/usr/bin/env python
 """GPU-box study behind tests/test_fullsize_gpu.py: codebook-index differences against the CPU oracle at the FULL benchmark
-geometry (x4, 128x128, batch 32 = 131072 VQ rows, default tie-heavy init) for several arithmetic variants of the engine,
-each classified by the ORACLE's own fp32 distances: a difference is "tie-equivalent" when the oracle's distance of our
+geometry (x4, 128x128, batch 32 = 131072 VQ rows, default tie-heavy init) for the engine's two GEMM paths, each
+classified by the ORACLE's own fp32 distances: a difference is "tie-equivalent" when the oracle's distance of our
 code is within `k` grid steps (ulp of A = sum z^2) of the oracle's best - i.e. the two codes are separated by less than
 the rounding noise of ANY fp32 evaluation order (the oracle itself moves this many rows when its thread count changes,
 profiles/oracle_selfcheck_r2.json).
 
     python scripts/flip_study.py > gpurun_out/flip_study.json       (about 3 minutes, mostly the CPU oracle)
+
+Another arithmetic variant, such as a K-slice length other than engine.cu's Ctx::SLICE_KB, is a second library build:
+add an entry whose environment sets FEMASR_LIB to that library.
 """
 import json
 import os
@@ -21,10 +24,6 @@ sys.path.insert(0, ROOT)
 
 VARIANTS = {
     "default (tensor-core, K-slice 256)": {},
-    "tensor-core, K-slice 128": {"FEMASR_TC_SLICE_KB": "2"},
-    "tensor-core, K-slice 64": {"FEMASR_TC_SLICE_KB": "1"},
-    "tensor-core, no K-slicing": {"FEMASR_TC_PRECISE": "0"},
-    "tensor-core, VQ on fp32 SIMT": {"FEMASR_VQ_FUSED": "0"},
     "fp32 FFMA path (gemm_path=0)": {"FEMASR_GEMM_PATH": "0"},
 }
 

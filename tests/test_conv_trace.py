@@ -8,14 +8,15 @@ policy, for every configuration and legal shape of tests/test_engine_plan.py and
   SiLU and K-slicing (slice_kb 4) wherever the launch has more than 4 k-blocks; behind it F8 for exactly the staged 3x3
   convs without a LayerNorm prologue whose weight has the F8 form, and the fast SiLU; the semantic branch and LPIPS in one
   pass without F8; every discriminator conv precise.
-- The trace is repeatable and independent of registered taps and conv captures."""
+- The trace is repeatable and independent of registered taps and conv captures.
+- Workspace bytes and traces ignore the environment variables that once selected other numerics."""
 import ctypes
 import json
 
 import pytest
 
 from femasr_b200 import lib
-from tests.test_engine_plan import CONFIGS, DIV, HEAD_SHAPES, HEADS, SHAPES
+from tests.test_engine_plan import CONFIGS, DIV, HEAD_SHAPES, HEADS, SHAPES, head_plan, plan
 from tests.test_gemm_matrix_gpu import ACCEPTED, CLASSES, SIMT_ONLY, SIMT_REFUSES
 
 I3 = ctypes.c_int * 3
@@ -218,6 +219,29 @@ def test_numerics_policy(built_lib, gemm_path):
                 assert r["f8"] == want_f8, f"{at}: f8 {r['f8']}, expected {want_f8}"
                 assert r["slice_kb"] == 0, at
                 assert r["prologue"] != "gn", f"{at}: exact SiLU behind the VQ"
+
+
+# environment variables that once selected other numerics, each with a value that did so
+FORMER_KNOBS = {"FEMASR_TC_PRECISE": "0", "FEMASR_FAST_SILU": "0", "FEMASR_VQ_FUSED": "0", "FEMASR_F8_CROSS": "0",
+                "FEMASR_TC_SLICE_KB": "2", "FEMASR_SEM_SLICE_KB": "4"}
+
+
+def sizing(gemm_path):
+    """Every configuration's and head's plan table (tests/test_engine_plan.py: workspace bytes, FLOPs) and sizing traces."""
+    L = lib.load()
+    return ({name: plan(L, name, gemm_path) for name in CONFIGS}, {name: head_plan(L, name, gemm_path) for name in HEADS},
+            {name: gen_traces(L, name, gemm_path) for name in CONFIGS},
+            {name: head_traces(L, name, gemm_path) for name in HEADS})
+
+
+@pytest.mark.parametrize("var", sorted(FORMER_KNOBS))
+def test_numerics_ignore_the_environment(built_lib, monkeypatch, var):
+    for v in FORMER_KNOBS:
+        monkeypatch.delenv(v, raising=False)
+    want = [sizing(gp) for gp in (0, 1)]
+    monkeypatch.setenv(var, FORMER_KNOBS[var])
+    for gp in (0, 1):
+        assert sizing(gp) == want[gp], f"{var}={FORMER_KNOBS[var]} changes the gemm_path {gp} plan"
 
 
 @pytest.mark.parametrize("gemm_path", [0, 1])

@@ -20,8 +20,9 @@ from tests.test_semantic import SEM_GOLDEN, SEM_IDS, load_sem_case
 pytestmark = pytest.mark.gpu
 # gemm_path 1 runs the VGG convs in ONE pass on the tensor cores, whose fp32 accumulator truncates: measured on an H100,
 # relu4_4 comes out biased by -7.8e-5 (relative, the same sign everywhere) and the loss, a mean of squares, by about twice
-# that (-1.6e-4 on hq_e512_sem_fwd_default, -8.7e-5 on hq_e512_sem_fwd).  K slices of 256 (FEMASR_SEM_SLICE_KB=4) cut
-# both tenfold; the branch only feeds a scalar loss, so the one-pass GEMM is kept and the bar covers its bias.
+# that (-1.6e-4 on hq_e512_sem_fwd_default, -8.7e-5 on hq_e512_sem_fwd).  K slices of 256 (measured with
+# FEMASR_SEM_SLICE_KB=4, a study knob since removed) cut both tenfold; the branch only feeds a scalar loss, so the
+# one-pass GEMM is kept and the bar covers its bias.
 SEM_RTOL = {0: 2e-5, 1: 3e-4}
 
 

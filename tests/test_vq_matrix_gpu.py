@@ -241,7 +241,7 @@ def test_vq_matrix(cuda, n_e, e_dim, rows, kind, k):
 
 @pytest.mark.parametrize("n_e,e_dim,rows,kind,k", [p for p in TABLE if p.values[2] != "131072"])
 def test_vq_select_matrix(cuda, n_e, e_dim, rows, kind, k):
-    """femasr_vq_select (gemm_path 0, FEMASR_VQ_FUSED=0) given the contract's C: exact."""
+    """femasr_vq_select (the VQ of gemm_path 0) given the contract's C: exact."""
     N = rows_of(rows)
     z, cb = make_case(n_e, e_dim, N, kind, k, seed=1000 + n_e + e_dim + abs(k))
     z, cb = z.to(cuda), cb.to(cuda)
