@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <atomic>
 #include <string>
 
 #include "femasr_b200.h"
@@ -36,7 +37,9 @@ inline int launch_status(const char* what) {
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
 // Per-device one-time state.  cudaFuncSetAttribute(MaxDynamicSharedMemorySize) and the SM count belong to a DEVICE, not
-// to the process: engines on several GPUs may live in one process (the reference surface is `.to(any device)`).
+// to the process: engines on several GPUs may live in one process (the reference surface is `.to(any device)`).  Engines
+// on one device may be driven from several host threads at once, so the caches are atomic: two threads that both find
+// a flag clear both make the (idempotent) runtime call, and a thread that finds it set knows the call has returned.
 constexpr int MAX_DEVICES = 64;
 inline int current_device() {
   int d = 0;
@@ -44,18 +47,19 @@ inline int current_device() {
   return d;
 }
 struct PerDeviceFlag {
-  bool set[MAX_DEVICES] = {};
-  bool& cur() { return set[current_device()]; }
+  std::atomic<bool> set[MAX_DEVICES] = {};
+  std::atomic<bool>& cur() { return set[current_device()]; }
 };
 inline int sm_count() {
-  static int counts[MAX_DEVICES] = {};
+  static std::atomic<int> counts[MAX_DEVICES] = {};
   const int d = current_device();
-  if (!counts[d]) {
-    int n = 0;
+  int n = counts[d].load();
+  if (!n) {
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d);
-    counts[d] = n > 0 ? n : 132;
+    n = n > 0 ? n : 132;
+    counts[d].store(n);
   }
-  return counts[d];
+  return n;
 }
 
 __host__ __device__ inline long cdiv(long a, long b) { return (a + b - 1) / b; }

@@ -84,19 +84,22 @@ __global__ void __launch_bounds__(256) in_conv_kernel(const float* __restrict__ 
 
 // out_conv: 3x3, Cin=64 -> 3.  The input tile (with halo) is staged in shared memory by coalesced 16-byte
 // loads (NHWC rows are contiguous), pixel stride padded to 68 floats so the per-thread float4 reads are
-// bank-conflict free; the 1728 weights sit in __constant__ memory (uniform across the warp -> FFMA with a
-// constant operand, no load instruction).  One thread per output pixel, tile = 4 rows x 32 cols.
+// bank-conflict free; the 9 * 64 * CO weights are staged after it and read as warp-uniform float4 broadcasts.  They come
+// from the caller's w on every launch, so engines on other streams or threads never see each other's weights.
+// One thread per output pixel, tile = 4 rows x 32 cols.
 constexpr int OC_CIN = 64, OC_TH = 4, OC_TW = 32, OC_PS = 68;   // pixel stride in floats
-__constant__ float c_outconv_w[9 * OC_CIN * 3];
-__constant__ float c_outconv_b[4];
+constexpr int OC_TILE = (OC_TH + 2) * (OC_TW + 2) * OC_PS;      // tile floats (a multiple of 4: the weights stay 16-byte aligned)
 
-// CO output channels (3: out_conv, 1: the discriminator's conv9); the weights use the first 9 * OC_CIN * CO floats
+// CO output channels (3: out_conv, 1: the discriminator's conv9); w: K-major packed [tap][c][co] (femasr_pack_weight)
 template <int CO>
-__global__ void __launch_bounds__(OC_TH * OC_TW) out_conv_kernel(const float* __restrict__ x, float* __restrict__ y,
+__global__ void __launch_bounds__(OC_TH * OC_TW) out_conv_kernel(const float* __restrict__ x, const float* __restrict__ w,
+                                                                 const float* __restrict__ bias, float* __restrict__ y,
                                                                  int B, int H, int W) {
-  extern __shared__ __align__(16) float tile[];      // [(OC_TH+2)][(OC_TW+2)][OC_PS]
+  extern __shared__ __align__(16) float tile[];      // [(OC_TH+2)][(OC_TW+2)][OC_PS], then the weights [9][OC_CIN][CO]
+  float* wsm = tile + OC_TILE;
   const int x0 = blockIdx.x * OC_TW, y0 = blockIdx.y * OC_TH, b = blockIdx.z;
   constexpr int TWH = OC_TW + 2, THH = OC_TH + 2;
+  for (int i = threadIdx.x; i < 9 * OC_CIN * CO; i += OC_TH * OC_TW) wsm[i] = __ldg(w + i);
   // cooperative halo load: (THH*TWH) pixels x 16 float4
   for (int i = threadIdx.x; i < THH * TWH * (OC_CIN / 4); i += OC_TH * OC_TW) {
     const int c4 = i % (OC_CIN / 4);
@@ -113,18 +116,23 @@ __global__ void __launch_bounds__(OC_TH * OC_TW) out_conv_kernel(const float* __
   const int ox = x0 + lx, oy = y0 + ly;
   float a[CO];
 #pragma unroll
-  for (int co = 0; co < CO; ++co) a[co] = c_outconv_b[co];
+  for (int co = 0; co < CO; ++co) a[co] = __ldg(bias + co);
 #pragma unroll 1
   for (int kh = 0; kh < 3; ++kh)
 #pragma unroll
     for (int kw = 0; kw < 3; ++kw) {
       const float* px = &tile[((ly + kh) * TWH + lx + kw) * OC_PS];
-      const float* wt = c_outconv_w + (kh * 3 + kw) * OC_CIN * CO;
+      const float* wt = wsm + (kh * 3 + kw) * OC_CIN * CO;
 #pragma unroll 4
       for (int c4 = 0; c4 < OC_CIN / 4; ++c4) {
         const float4 v = *reinterpret_cast<const float4*>(px + c4 * 4);
         const float vv[4] = {v.x, v.y, v.z, v.w};
-        const float* wk = wt + c4 * 4 * CO;
+        float wk[4 * CO];                              // the 4 channels' weights [e][co]: CO float4 broadcasts
+#pragma unroll
+        for (int j = 0; j < CO; ++j) {
+          const float4 q = *reinterpret_cast<const float4*>(wt + (c4 * CO + j) * 4);
+          wk[4 * j] = q.x; wk[4 * j + 1] = q.y; wk[4 * j + 2] = q.z; wk[4 * j + 3] = q.w;
+        }
 #pragma unroll
         for (int e = 0; e < 4; ++e)
 #pragma unroll
@@ -260,17 +268,14 @@ extern "C" int femasr_in_conv_pad_weight(const float* w_oihw, float* w_padded, i
 
 template <int CO>
 static int out_conv_simt(const float* x, const float* w, const float* bias, float* y, int B, int H, int W, cudaStream_t st) {
-  // weights travel through __constant__ memory; refreshed per call (stream-ordered) so several engines can coexist
-  FEMASR_CUDA(cudaMemcpyToSymbolAsync(c_outconv_w, w, sizeof(float) * 9 * OC_CIN * CO, 0, cudaMemcpyDeviceToDevice, st));
-  FEMASR_CUDA(cudaMemcpyToSymbolAsync(c_outconv_b, bias, sizeof(float) * CO, 0, cudaMemcpyDeviceToDevice, st));
-  constexpr int smem = (OC_TH + 2) * (OC_TW + 2) * OC_PS * (int)sizeof(float);
+  constexpr int smem = (OC_TILE + 9 * OC_CIN * CO) * (int)sizeof(float);
   static PerDeviceFlag attr_set;
   if (!attr_set.cur()) {
     FEMASR_CUDA(cudaFuncSetAttribute(out_conv_kernel<CO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_set.cur() = true;
   }
   dim3 grid((unsigned)cdiv(W, OC_TW), (unsigned)cdiv(H, OC_TH), B);
-  out_conv_kernel<CO><<<grid, OC_TH * OC_TW, smem, st>>>(x, y, B, H, W);
+  out_conv_kernel<CO><<<grid, OC_TH * OC_TW, smem, st>>>(x, w, bias, y, B, H, W);
   return launch_status("out_conv_kernel");
 }
 
@@ -291,7 +296,6 @@ constexpr int OM_TH = 8, OM_TW = 30, OM_PX = 32, OM_PB = 144;     // halo pixels
 constexpr int OM_PLANE = (OM_TH + 2) * OM_PX * OM_PB;             // 46080 B per fp16 plane
 constexpr int OM_SMEM = 2 * OM_PLANE + OM_TH * OM_PX * 9 * (int)sizeof(float);
 constexpr float OM_WSCALE = 256.0f;                               // weights * 2^8: keeps the lo plane out of fp16 subnormals
-__device__ uint32_t g_outconv_bfrag[3 * 4 * 2 * 2 * 2 * 32];       // [kh][kc][nt][plane][reg][lane] B fragments (refreshed per call)
 
 // (x, y) -> packed fp16 pairs hi = rn(v), lo = rn(v - hi), saturating at +-65504 like the big GEMMs' operand staging
 __device__ __forceinline__ void oc_split2(float x, float y, uint32_t& hi, uint32_t& lo) {
@@ -300,32 +304,29 @@ __device__ __forceinline__ void oc_split2(float x, float y, uint32_t& hi, uint32
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(y - hf.y), "f"(x - hf.x));
 }
 
-// w: K-major packed [tap][c][co] fp32 (femasr_pack_weight), CO output channels (3 or 1): the folded N = 3 * CO columns
-// fill one (CO 1) or two (CO 3) 8-wide n-tiles.  One thread per (kh, kc, nt, reg, lane).
+// This lane's B fragment register `reg` of tap row kh, 16-channel chunk kc and n-tile nt, as split fp16 (hi, lo) of the
+// weights * OM_WSCALE.  w: K-major packed [tap][c][co] fp32 (femasr_pack_weight), CO output channels (3 or 1): the folded
+// N = 3 * CO columns fill one (CO 1) or two (CO 3) 8-wide n-tiles.  Built from the caller's w in every CTA (L2-resident
+// loads), so engines on other streams or threads never see each other's weights.
 template <int CO>
-__global__ void out_conv_bfrag_kernel(const float* __restrict__ w) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= 3 * 4 * 2 * 2 * 32) return;
-  const int lane = idx & 31, reg = (idx >> 5) & 1, nt = (idx >> 6) & 1, kc = (idx >> 7) & 3, kh = idx >> 9;
+__device__ __forceinline__ void oc_bfrag(const float* __restrict__ w, int kh, int kc, int nt, int reg, int lane, uint32_t& hi,
+                                         uint32_t& lo) {
   const int g = lane >> 2, cq = lane & 3;
   const int n = nt * 8 + g;                       // column = kw*CO + co
   float v0 = 0.f, v1 = 0.f;
   if (n < 3 * CO) {
     const int kw = n / CO, co = n - CO * kw;
     const int ch = 16 * kc + 2 * cq + 8 * reg;    // B fragment: b0 = k 2c,2c+1; b1 = k 2c+8,2c+9
-    v0 = w[(((kh * 3 + kw) * OC_CIN) + ch) * CO + co] * OM_WSCALE;
-    v1 = w[(((kh * 3 + kw) * OC_CIN) + ch + 1) * CO + co] * OM_WSCALE;
+    v0 = __ldg(w + (((kh * 3 + kw) * OC_CIN) + ch) * CO + co) * OM_WSCALE;
+    v1 = __ldg(w + (((kh * 3 + kw) * OC_CIN) + ch + 1) * CO + co) * OM_WSCALE;
   }
-  uint32_t hi, lo;
   oc_split2(v0, v1, hi, lo);
-  const int base = (((kh * 4 + kc) * 2 + nt) * 2) * 2;        // [plane][reg]
-  g_outconv_bfrag[(base + 0 * 2 + reg) * 32 + lane] = hi;
-  g_outconv_bfrag[(base + 1 * 2 + reg) * 32 + lane] = lo;
 }
 
 template <int CO>
-__global__ void __launch_bounds__(OM_TH * 32, 2) out_conv_mma_kernel(const float* __restrict__ x, const float* __restrict__ bias,
-                                                                     float* __restrict__ y, int B, int H, int W) {
+__global__ void __launch_bounds__(OM_TH * 32, 2) out_conv_mma_kernel(const float* __restrict__ x, const float* __restrict__ w,
+                                                                     const float* __restrict__ bias, float* __restrict__ y,
+                                                                     int B, int H, int W) {
   constexpr int NC = 3 * CO, NT = (NC + 7) / 8;     // folded columns kw*CO + co, 8-wide n-tiles
   extern __shared__ __align__(16) uint8_t om_smem[];
   uint8_t* plane_hi = om_smem;
@@ -377,11 +378,7 @@ __global__ void __launch_bounds__(OM_TH * 32, 2) out_conv_mma_kernel(const float
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          const int base = (((kh * 4 + kc) * 2 + nt) * 2) * 2;
-          bh[kc][nt][r] = g_outconv_bfrag[(base + r) * 32 + lane];
-          bl[kc][nt][r] = g_outconv_bfrag[(base + 2 + r) * 32 + lane];
-        }
+        for (int r = 0; r < 2; ++r) oc_bfrag<CO>(w, kh, kc, nt, r, lane, bh[kc][nt][r], bl[kc][nt][r]);
     const int row = warp + kh;                    // halo row feeding output row `warp` through tap row kh
 #pragma unroll
     for (int kc = 0; kc < 4; ++kc)
@@ -435,14 +432,13 @@ __global__ void __launch_bounds__(OM_TH * 32, 2) out_conv_mma_kernel(const float
 
 template <int CO>
 static int out_conv_mma(const float* x, const float* w, const float* bias, float* y, int B, int H, int W, cudaStream_t st) {
-  out_conv_bfrag_kernel<CO><<<6, 256, 0, st>>>(w);     // stream-ordered refresh of the B fragments (several engines can coexist)
   static PerDeviceFlag attr_set;
   if (!attr_set.cur()) {
     FEMASR_CUDA(cudaFuncSetAttribute(out_conv_mma_kernel<CO>, cudaFuncAttributeMaxDynamicSharedMemorySize, OM_SMEM));
     attr_set.cur() = true;
   }
   dim3 grid((unsigned)cdiv(W, OM_TW), (unsigned)cdiv(H, OM_TH), B);
-  out_conv_mma_kernel<CO><<<grid, OM_TH * 32, OM_SMEM, st>>>(x, bias, y, B, H, W);
+  out_conv_mma_kernel<CO><<<grid, OM_TH * 32, OM_SMEM, st>>>(x, w, bias, y, B, H, W);
   return launch_status("out_conv_mma_kernel");
 }
 

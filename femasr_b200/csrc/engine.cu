@@ -6,6 +6,7 @@
 #include <cmath>
 #include <cstring>
 #include <map>
+#include <mutex>
 #include <set>
 #include <string>
 #include <vector>
@@ -443,13 +444,16 @@ struct Ctx {
   }
 
   // FEMASR_PROFILE_DETAIL=1: per-shape kernel labels in the profile ("tc_igemm:k3:64->64@512x512"); the strings are
-  // interned for the life of the process because the profile records keep only the pointer
+  // interned for the life of the process because the profile records keep only the pointer.  The set is shared by the
+  // handles of every host thread, hence the lock (std::set nodes never move, so a returned pointer stays valid).
   const char* detail_name(const char* base, int k, int Cin, int Cout, int H, int W, int up, int stride, int slice) {
     static const bool detail = [] { const char* e = getenv("FEMASR_PROFILE_DETAIL"); return e && atoi(e) != 0; }();
     if (!detail || !net->profile) return base;
+    static std::mutex mu;
     static std::set<std::string> names;
     std::string s = std::string(base) + ":k" + std::to_string(k) + ":" + std::to_string(Cin) + "->" + std::to_string(Cout) + "@" +
                     std::to_string(H) + "x" + std::to_string(W) + (up ? ":up" : "") + (stride == 2 ? ":s2" : "") + (slice ? ":sliced" : "");
+    std::lock_guard<std::mutex> lock(mu);
     return names.insert(s).first->c_str();
   }
 

@@ -7,6 +7,10 @@
  * Every entry point returns 0 on success or a negative femasr_status; femasr_last_error() gives
  * the message (thread-local).  Nothing here owns caller memory; nothing falls back to the CPU.
  *
+ * Concurrency: engines (and the standalone kernels) may run concurrently on separate streams and host threads of one
+ * device; no kernel keeps state in library-global device memory.  One handle is used by one host thread at a time,
+ * because its trace, graph captures and profile are per handle.
+ *
  * Data layout: activations between kernels are NHWC fp32 ([B,H,W,C]; Swin tokens [B,HW,C] are the
  * same bytes).  Images at the public boundary are NCHW fp32 like the reference's tensors.
  */
@@ -401,9 +405,7 @@ int femasr_out_conv3x3(const float* x_nhwc, const float* w, const float* bias, f
                        int H, int W, int Cin, void* stream);
 /* Same contract on warp-level tensor cores (mma.sync, 3-term split fp16; the three horizontal taps folded into N):
  * fp32-grade accuracy (not ATen-identical rounding), used by gemm_path 1.
- * Both out_conv entry points stage the 1728 weights in library-global device memory (`__constant__` / fragment
- * buffer) that is refreshed by every call in stream order: calls issued on DIFFERENT streams must not overlap
- * (one engine handle = one host thread = one stream at a time, see the threading note in INTEGRATION.md). */
+ * Both kernels read w and bias through the pointers of each call, so calls on different streams may overlap. */
 int femasr_out_conv3x3_mma(const float* x_nhwc, const float* w, const float* bias, float* y_nchw, int B,
                            int H, int W, int Cin, void* stream);
 /* The same two kernels for a head of Cout = 3 (out_conv) or 1 (UNetDiscriminatorSN.conv9) output channels:

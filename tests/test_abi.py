@@ -3,6 +3,7 @@ without a GPU the product path fails loudly instead of falling back."""
 import ctypes
 import os
 import re
+import subprocess
 
 import pytest
 import torch
@@ -25,6 +26,44 @@ def test_library_exports_every_declared_symbol(built_lib):
         assert hasattr(dll, n), f"{n} declared in the header but not exported"
     assert sorted(lib.SIGNATURES) == names, "femasr_b200/lib.py SIGNATURES out of sync with the header"
     assert lib.load().femasr_abi_version() == lib.ABI_VERSION == 4
+
+
+WRITABLE_DEVICE_SECTIONS = (".nv.global", ".nv.global.init", ".nv.constant3")
+_HEX = r"(?:0x)?[0-9a-f]+"
+_SECTION_ROW = re.compile(rf"^\s*({_HEX})\s+{_HEX}\s+{_HEX}\s+{_HEX}\s+{_HEX}\s+[A-Z_]+\s+{_HEX}\s+{_HEX}\s+{_HEX}\s+(\S+)$")
+_SYMBOL_ROW = re.compile(rf"^\s*{_HEX}\s+{_HEX}\s+{_HEX}\s+({_HEX})\s+{_HEX}\s+({_HEX})\s+(\S+)$")
+
+
+def device_globals(elf_dump):
+    """{symbol: section} of every symbol `cuobjdump -elf` lists in a writable library-global device section (__device__
+    variables land in .nv.global / .nv.global.init, __constant__ ones in .nv.constant3), over every cubin in the dump."""
+    found = {}
+    for cubin in elf_dump.split("Fatbin elf code:")[1:]:
+        sections, in_symtab = {}, False
+        for line in cubin.splitlines():
+            if line.startswith(".section"):
+                in_symtab = line.split()[1] == ".symtab"
+            elif not in_symtab and (m := _SECTION_ROW.match(line)):       # Index Offset Size ES Align Type Flags Link Info Name
+                sections[int(m[1], 16)] = m[2]
+            elif in_symtab and (m := _SYMBOL_ROW.match(line)):            # index value size info other shndx name
+                sec = sections.get(int(m[2], 16), "")
+                if sec in WRITABLE_DEVICE_SECTIONS and (int(m[1], 16) & 0xF) != 3:   # STT_SECTION rows name the section
+                    found[m[3]] = sec
+    return found
+
+
+def test_library_has_no_device_globals(built_lib):
+    """Engines on separate streams or host threads of one device run concurrently, so no kernel may keep its operands in
+    library-global device memory: every weight travels through the handle's own buffers.  A __device__ or __constant__
+    variable in the library is state shared by every engine in the process."""
+    from femasr_b200 import build
+    cuobjdump = os.path.join(os.path.dirname(build._nvcc()), "cuobjdump")
+    if not os.path.exists(cuobjdump):
+        pytest.skip("cuobjdump not found beside nvcc")
+    dump = subprocess.run([cuobjdump, "-elf", built_lib], check=True, capture_output=True, text=True).stdout
+    assert dump.count("Fatbin elf code:") >= len(build.sources()), "cuobjdump listed fewer cubins than sources"
+    found = device_globals(dump)
+    assert not found, "library-global device variables: " + ", ".join(f"{k} ({v})" for k, v in sorted(found.items()))
 
 
 def test_argument_validation_without_gpu(built_lib):

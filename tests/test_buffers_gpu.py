@@ -11,7 +11,8 @@ outside the buffers a call was given.
   with 1 MiB of 0xA5 on each side, and every output (and tap) inside its own guards, prefilled with a NaN pattern.
   Afterwards the guards are intact and no output element still holds the prefill.
 - Sequences on one stream: shapes and entry points alternating on one handle and workspace; generator, discriminator and
-  LPIPS interleaved (they share the out_conv kernels' library-global weights); a captured graph replayed around them.
+  LPIPS interleaved (the generator's out_conv and the discriminator's conv9 run the same kernels with different weights);
+  a captured graph replayed around them.  tests/test_concurrency_gpu.py runs them on separate streams and threads.
 - The kernels outside the arena (test(), test_tile(), sr_uint8() and out_conv's writes into the caller's y) against
   exact references, inside guard bands."""
 import ctypes as C
@@ -118,13 +119,17 @@ def poison_matrix(what, handle, need, specs, launch, dev):
 _SD = {}
 
 
-def make_gen(name, gemm_path, dev):
+def make_gen(name, gemm_path, dev, seed=90, head=1.0):
+    """A generator of configuration `name` with seeded weights; `head` scales its out_conv weight and bias."""
     scale, cbs, sem, _tap = CONFIGS[name]
-    key = (scale, str(cbs), sem)
+    key = (scale, str(cbs), sem, seed, head)
     if key not in _SD:
         if len(_SD) > 1:
             _SD.clear()
-        _SD[key] = random_state_dict(scale, cbs[0][2], seed=90, init="perturbed", codebooks=cbs, semantic=sem)
+        sd = random_state_dict(scale, cbs[0][2], seed=seed, init="perturbed", codebooks=cbs, semantic=sem)
+        if head != 1.0:
+            sd = {k: v * head if k.startswith("out_conv.") else v for k, v in sd.items()}
+        _SD[key] = sd
     net = NativeNet(scale, cbs[0][1], cbs[0][2], gemm_path=gemm_path, codebooks=cbs, use_semantic_loss=sem)
     net.sd = _SD[key]
     net.load_state_dict(net.sd, dev)
@@ -218,9 +223,11 @@ def test_generator_poison_and_guards(cuda, name, gemm_path):
 
 
 # ------------------------------------------------------------------------------------------------ discriminator, LPIPS
-def make_disc(skip, gemm_path, dev, seed=91):
+def make_disc(skip, gemm_path, dev, seed=91, head=1.0):
+    """A discriminator with seeded weights; `head` scales its conv9 (Cout 1) weight and bias."""
     d = NativeDisc(skip_connection=bool(skip), gemm_path=gemm_path)
-    d.load_state_dict(random_disc_state_dict(seed), dev)
+    sd = random_disc_state_dict(seed)
+    d.load_state_dict({k: v * head if k.startswith("conv9.") else v for k, v in sd.items()}, dev)
     return d
 
 
@@ -283,8 +290,8 @@ def run_entry(need, specs, launch, dev, ws=None):
 
 
 def check_head(net, y, dec2, tag):
-    """y against out_conv in fp64 on the dec2 tap: a reference that does not go through the library-global out_conv
-    weights (bars of tests/test_ops_gpu.py::test_in_conv_out_conv)."""
+    """y against out_conv in fp64 on the dec2 tap with this net's own weights: a head that read another engine's weights
+    misses by orders of magnitude (bars of tests/test_ops_gpu.py::test_in_conv_out_conv)."""
     sd = net.sd
     want = F.conv2d(G.nchw(dec2).double().cpu(), sd["out_conv.weight"].double(), sd["out_conv.bias"].double(), padding=1)
     err = (y.double().cpu() - want).abs().max().item()
@@ -330,28 +337,34 @@ def test_sequences_one_handle(cuda, gemm_path):
     solo.close()
 
 
+def gen_dec2_entry(gen, x):
+    """(need, specs, launch) of a generator forward that also writes the dec2 tap, the input of out_conv."""
+    B, _, H, W = x.shape
+    specs, launch = gen_forward(gen, x, B, H, W, False)
+    tshape = gen.tap_shapes(B, H, W)["dec2"]
+    specs["tap:dec2"] = (torch.float32, tshape)
+
+    def launch_tap(p, ws, n):
+        L.check(gen.lib.femasr_net_set_tap(gen._h, b"dec2", p["tap:dec2"], math.prod(tshape)))
+        try:
+            return launch(p, ws, n)
+        finally:
+            gen.lib.femasr_net_set_tap(gen._h, b"dec2", None, 0)
+    return gen_need(gen, B, H, W, False), specs, launch_tap
+
+
 @pytest.mark.parametrize("gemm_path", [0, 1])
 def test_engines_interleaved(cuda, gemm_path):
     """Generator -> discriminator -> generator -> LPIPS -> generator on one stream: each result equals that engine's
     solo result, and the generator's y equals out_conv of its dec2 tap in fp64.  The generator's out_conv (Cout 3) and
-    the discriminator's conv9 (Cout 1) share the SIMT kernel's __constant__ weights (gemm_path 0) and the mma kernel's
-    global B fragments (gemm_path 1), both refreshed in stream order on every call."""
+    the discriminator's conv9 (Cout 1) run the same SIMT (gemm_path 0) or mma (gemm_path 1) kernels, each call with its
+    own weights."""
     gen = make_gen("x4_e256", gemm_path, cuda)
     d = make_disc(1, gemm_path, cuda)
     m = make_lpips("vgg", gemm_path, cuda)
     B, H, W = RAGGED[4]
     x = torch.rand(B, 3, H, W, generator=torch.Generator().manual_seed(5)).to(cuda)
-    gspecs, glaunch = gen_forward(gen, x, B, H, W, False)
-    gspecs["tap:dec2"] = (torch.float32, gen.tap_shapes(B, H, W)["dec2"])
-    tshape = gspecs["tap:dec2"][1]
-
-    def glaunch_tap(p, ws, n):
-        L.check(gen.lib.femasr_net_set_tap(gen._h, b"dec2", p["tap:dec2"], math.prod(tshape)))
-        try:
-            return glaunch(p, ws, n)
-        finally:
-            gen.lib.femasr_net_set_tap(gen._h, b"dec2", None, 0)
-    gentry = (gen_need(gen, B, H, W, False), gspecs, glaunch_tap)
+    gentry = gen_dec2_entry(gen, x)
     dentry = disc_entry(d, (x * 2 - 1).contiguous())
     x1 = torch.rand(B, 3, H, W, generator=torch.Generator().manual_seed(6)).to(cuda)
     mentry = lpips_entry(m, x, x1, 1)
@@ -504,8 +517,8 @@ OUT_SHAPES = {0: ((3, 31), (4, 32), (5, 33), (1, 1), (9, 65)), 1: ((7, 29), (8, 
 
 @pytest.mark.parametrize("mma", [0, 1])
 def test_out_conv_guarded(cuda, mma):
-    """femasr_out_conv3x3_n writes the caller's NCHW y: Cout 3 and Cout 1 alternating (they share the library-global
-    weights), at sizes one below, at and one above the 4x32 (SIMT) and 8x30 (mma) tiles, B = 3, inside guard bands."""
+    """femasr_out_conv3x3_n writes the caller's NCHW y: Cout 3 and Cout 1 alternating (each call with its own weights),
+    at sizes one below, at and one above the 4x32 (SIMT) and 8x30 (mma) tiles, B = 3, inside guard bands."""
     lib = L.load()
     B = 3
     for i, (H, W) in enumerate(OUT_SHAPES[mma]):
